@@ -3,7 +3,7 @@
 // Package allocategpu: the Go side of libvcalloc.so (include/vcalloc.h) for volcano's scheduler.
 //
 // NOT COMPILED in the build image of this repository (no Go toolchain there); written against
-// volcano.sh/volcano/pkg/scheduler at the revision under /root/reference. It is the complete marshalling
+// volcano.sh/volcano/pkg/scheduler. It is the complete marshalling
 // ("encodeSession") the Python mirror volcano_b200/snapshot.py::encode_cluster implements and the parity tests
 // drive; field by field the two do the same thing, and every array below is one field of include/vcalloc.h.
 //

@@ -21,6 +21,7 @@ cluster / max-over-ranks kernel time. N scheduler replicas (one cluster per GPU)
 from __future__ import annotations
 
 import argparse
+import atexit
 import json
 import os
 import statistics
@@ -45,7 +46,7 @@ def _peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not measured)"
 
 
 class ClockSampler:
@@ -62,6 +63,7 @@ class ClockSampler:
         try:
             self.p = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.FIELDS}", "--format=csv,noheader,nounits",
                                        "-lms", "100", "-i", str(self.gpu)], stdout=self.f, stderr=subprocess.DEVNULL)
+            atexit.register(self.p.kill)  # the sampler must not outlive a run that fails before stop()
         except Exception:
             self.p = None
 
@@ -166,6 +168,28 @@ def compare_placements(res, oracle_results):
     return out
 
 
+DUMP_LIMIT_BYTES = (64 << 20) - (64 << 10)  # 64 MB with room for the .npy headers
+
+
+def dump_outputs(res, out_dir):
+    """What a caller of the timed path receives from one cycle (decisions, visits, fit errors) as DIR/<table>_<field>.npy in
+    float64 (every integer field is exact there). Past 64 MB in all, each table keeps a fixed, seeded sample of its rows and
+    stores their indices as DIR/<table>_row.npy, so two builds given the same arguments dump the same rows."""
+    tables = {"decision": {f: res.decisions[f] for f in res.decisions.dtype.names},
+              "visit": {f: res.visits[f] for f in res.visits.dtype.names},
+              "fit_error": {"task": res.fit_errors}}
+    total = sum(a.size * 8 for cols in tables.values() for a in cols.values())
+    os.makedirs(out_dir, exist_ok=True)
+    for seed, (table, cols) in enumerate(tables.items()):
+        if total > DUMP_LIMIT_BYTES:
+            n = len(next(iter(cols.values())))
+            keep = int(n * DUMP_LIMIT_BYTES / total * len(cols) / (len(cols) + 1))
+            rows = np.sort(np.random.default_rng(seed).choice(n, size=keep, replace=False))
+            cols = {"row": rows, **{f: a[rows] for f, a in cols.items()}}
+        for f, a in cols.items():
+            np.save(os.path.join(out_dir, f"{table}_{f}.npy"), np.asarray(a, dtype=np.float64))
+
+
 def config_dict(name, world):
     """The same keys in both arms (the driver compares the dicts)."""
     return {"workload": workload_desc(name),
@@ -252,6 +276,8 @@ def multi_gpu_arm(args, rank, world, local):
         placed += int(cnt[0].item())
         n_steps += int(cnt[1].item())
     t_dev = sum(dev_ms) / 1e3
+    if args.dump_outputs and rank == 0:
+        dump_outputs(res, args.dump_outputs)
     # ---- e2e: host buffers -> upload on every rank -> one session -> decisions on rank 0's host ----
     torch.cuda.synchronize(); dist.barrier()
     t0 = time.perf_counter()
@@ -362,6 +388,8 @@ def main():
     ap.add_argument("--impl", default="b200")
     ap.add_argument("--workload", default=WORKLOAD)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed cycle's decisions, visits and fit errors "
+                    "as DIR/*.npy (float64)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -387,7 +415,7 @@ def main():
     cfg = CONFIGS[args.workload]
     snap = make_snapshot(cfg, seed=cfg.seed + rank)  # every rank its own cluster shard of the same shape
     eng = engine.Engine(snap, device=local)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -415,6 +443,8 @@ def main():
         n_steps += res.stats["n_steps"]
     barrier()
     t_dev = sum(dev_ms) / 1e3
+    if args.dump_outputs and rank == 0:
+        dump_outputs(res, args.dump_outputs)
     # ---- e2e: host buffers -> upload -> allocate -> decisions on the host ------------------------
     barrier()
     t0 = time.perf_counter()
@@ -462,9 +492,6 @@ def main():
             peak, how = _peaks()
             ach = nbytes / (expand_ms * 1e-3) / 1e9
             traffic = None
-            tp = os.path.join(ROOT, "profiles", "r01_k1_expand_ncu.json")
-            if os.path.exists(tp) and args.workload == WORKLOAD:
-                traffic = json.load(open(tp)).get("traffic_bytes_per_launch")  # dram read+write, ncu --set full
             # the kernel is ~99.8 % stores: next to the (read+write) copy peak of MEASURED_PEAKS.json also measure a
             # write-only stream in this run (SURVEY §8d): cudaMemset-class fill of an 8 GB f64 buffer, best of 5
             wpeak = None

@@ -1,9 +1,9 @@
 /*
- * vcalloc.h — C ABI of libvcalloc.so: the B200-native replacement for Volcano's
+ * vcalloc.h — C ABI of libvcalloc.so: the GPU-native replacement for Volcano's
  * per-cycle `allocate` hot path.
  *
  * Every entry point below is what a cgo shim inside the reference would bind
- * (INTEGRATION.md shows the shim).  Citations are into /root/reference/pkg/scheduler
+ * (INTEGRATION.md shows the shim).  Citations are into volcano's pkg/scheduler
  * unless a full path is given.
  *
  *   reference interface replaced                         entry point here

@@ -14,7 +14,7 @@
 // published v1.35 algorithm and is pinned by the reference only at placement level:
 // for those numeric values parity is UNPINNED (SURVEY.md §8c).
 //
-// Citations are into /root/reference/pkg/scheduler unless a full path is given.
+// Citations are into volcano's pkg/scheduler unless a full path is given.
 //
 // Canonical determinism contract (SURVEY.md §7.0-2, §8c): tie-break = lowest NodeList index
 // among max-score nodes (the reference picks uniformly at random, util/scheduler_helper.go:

@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a, loads, exports every symbol of include/vcalloc.h, and — on a box
+"""The C-ABI library builds for sm_90a, loads, exports every symbol of include/vcalloc.h, and — on a box
 without a GPU — refuses to compute instead of falling back to a CPU path."""
 import ctypes as C
 import os

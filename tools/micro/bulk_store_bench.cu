@@ -1,4 +1,4 @@
-// How fast can shared->global bulk copies write HBM?  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o bulk_store_bench bulk_store_bench.cu
+// How fast can shared->global bulk copies write HBM?  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o bulk_store_bench bulk_store_bench.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>
@@ -40,7 +40,7 @@ int main() {
     printf("%-60s %.3f ms  %.0f GB/s  (%s)\n", name, ms, N * T * 8 / ms / 1e6, cudaGetErrorString(cudaGetLastError()));
   };
   time([&] { cudaMemsetAsync(out, 0, N * T * 8); }, "cudaMemsetAsync");
-  time([&] { k_plain<<<148 * 16, 256>>>((double2 *)out, N * T / 2); }, "plain st.cs double2, grid-stride");
+  time([&] { k_plain<<<132 * 16, 256>>>((double2 *)out, N * T / 2); }, "plain st.cs double2, grid-stride");
   for (int issuers : {1, 4}) for (int chunk : {5000, 10000}) for (int rows : {64, 16}) {
     cudaFuncSetAttribute(k_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, chunk * 8);
     dim3 grid((unsigned)(N / chunk), (unsigned)(T / rows));

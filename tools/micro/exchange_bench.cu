@@ -1,6 +1,6 @@
 // Micro-benchmark of the intra-GPU all-gather used by the commit kernels: G persistent CTAs, each posts one
 // 16-byte self-tagged record per round and reads everybody's. Prints cycles per round for several layouts.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o exchange_bench exchange_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o exchange_bench exchange_bench.cu
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <cstdio>

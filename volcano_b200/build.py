@@ -1,4 +1,4 @@
-"""In-tree build of libvcalloc.so for sm_100a (nvcc cross-compiles without a GPU)."""
+"""In-tree build of libvcalloc.so for sm_90a (nvcc cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -7,7 +7,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvcalloc.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

@@ -88,8 +88,8 @@ struct SpecNodeView {
 
 // Warp arg-max of (score, node) with the canonical tie-break plus the candidate count, for the one-category record of
 // the plain instance: four hardware reductions instead of the eight of local_warp_reduce (no soft-taint maximum, no
-// topology pair, no sampling position). Measured on B200: every warp-wide collective on this path costs ~300 cycles
-// (a 20-shuffle butterfly 5.6 k, the eight-op version 2.4 k), and three reductions sit on the per-task critical path.
+// topology pair, no sampling position). Every warp-wide collective adds its latency here, and three reductions sit on the
+// per-task critical path.
 __device__ __forceinline__ void simple_warp_reduce(Local &l) {
   constexpr unsigned FULLM = 0xffffffffu;
   const bool valid = l.node[0] >= 0;

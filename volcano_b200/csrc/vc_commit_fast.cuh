@@ -902,8 +902,8 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
   auto run_states = [&]() {
     const int L = F.run_L;
     // Evaluation slots in an order that fills the four SM sub-partitions one warp each before doubling up (a warp's
-    // sub-partition is warp % 4; fp64 instructions cost the sub-partition's pipe ~8 cycles each whatever the number of
-    // active lanes, tools/micro/fp64_latency.cu): warps 1, 3, 6, 4, then 5, 7; warp 2 (runner-up first) comes last.
+    // sub-partition is warp % 4; an fp64 instruction occupies the sub-partition's pipe whatever the number of
+    // active lanes, tools/micro/fp64_latency.cu measures it): warps 1, 3, 6, 4, then 5, 7; warp 2 (runner-up first) comes last.
     int e = warp - 1;
     if (nwarps == 8) e = warp == 1 ? 0 : warp == 3 ? 1 : warp == 6 ? 2 : warp == 4 ? 3 : warp == 5 ? 4 : warp == 7 ? 5 : 6;
     else if (warp == 2) e = nwarps - 2;

@@ -2,7 +2,7 @@
 // shared by the dense score-matrix kernel (K1) and the persistent commit kernel (K2).
 //
 // Everything here is fp64 / int arithmetic written in the exact operation order of the
-// reference (file:line cited per function, paths relative to /root/reference/pkg/scheduler);
+// reference (file:line cited per function, paths relative to volcano's pkg/scheduler);
 // the translation unit is compiled with -fmad=false so no mul+add is contracted.
 #pragma once
 #include <cuda_runtime.h>

@@ -352,11 +352,12 @@ __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, in
   }
   __syncthreads();
   if (warp == 0) {
-    int hp = 0;  // lane l walks warp l's list
-    unsigned long long ck = l_key[lane][0];
-    int cn = l_node[lane][0];
+    // lane l walks warp l's list; its head is read at the top of every step (advancing the index and reloading inside the
+    // branch below was compiled for sm_90a into a load of the slot after the new head, which dropped candidates)
+    int hp = 0;
     for (int it = 0; it < EV_PICK_K; ++it) {
-      unsigned long long gk = ck;
+      const int cn = hp < EV_PICK_K ? l_node[lane][hp] : -1;
+      unsigned long long gk = hp < EV_PICK_K ? l_key[lane][hp] : 0ull;
       int gn = cn;
       for (int o = 16; o; o >>= 1) {
         const unsigned long long ok = __shfl_xor_sync(0xffffffffu, gk, o);
@@ -365,11 +366,7 @@ __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, in
       }
       if (gn < 0) break;
       if (lane == 0) { s_pick[it] = gn; p.cand[gn] = 2; }
-      if (cn == gn) {
-        hp += 1;
-        ck = hp < EV_PICK_K ? l_key[lane][hp] : 0ull;
-        cn = hp < EV_PICK_K ? l_node[lane][hp] : -1;
-      }
+      if (cn == gn) hp += 1;
     }
   }
   __syncthreads();

@@ -1,4 +1,4 @@
-// vc_kernels.cuh — the CUDA kernels of libvcalloc.so (sm_100a).
+// vc_kernels.cuh — the CUDA kernels of libvcalloc.so (sm_90a).
 //
 //  k_class_static   K0  class x node static predicate / static score word (session open)
 //  k_group_eval     K1a group x node dense evaluation on the opening snapshot

@@ -1,5 +1,5 @@
 // vcalloc.cu — libvcalloc.so: C ABI (include/vcalloc.h) + host orchestration of the CUDA kernels.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -fmad=false -std=c++17
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false -std=c++17
 //             -Xcompiler -fPIC -shared vcalloc.cu -o libvcalloc.so          (volcano_b200/build.py)
 // There is no CPU path in this library: every entry point that computes needs a CUDA device.
 #include <cuda_runtime.h>
@@ -357,7 +357,7 @@ int build_devconf(vc_snapshot *s, const vc_nodes *nd) {
 // smallest launch geometry that keeps one node per thread when possible
 void choose_geometry(vc_snapshot *s) {
   const int nloc = s->dd.node_end - s->dd.node_begin;
-  int ctas = g_sm_count > 0 ? g_sm_count : 148;
+  int ctas = g_sm_count > 0 ? g_sm_count : 132;
   if (g_tun.commit_ctas > 0) ctas = g_tun.commit_ctas;
   int block = 128;
   if (g_tun.commit_threads > 0) block = std::max(128, std::min(256, g_tun.commit_threads / 32 * 32));
@@ -367,7 +367,7 @@ void choose_geometry(vc_snapshot *s) {
   int npc = (nloc + ctas - 1) / ctas;
   npc = std::max(32, (npc + 31) / 32 * 32);
   // mid-sized clusters on one GPU: four full warps of nodes per CTA (one per SM sub-partition in a sweep) and fewer slots to
-  // gather beat three warps on more CTAs (10k nodes: 79 x 128 instead of 105 x 96, +2.7 % at cfg2, +1.7 % at cfg3)
+  // gather beat three warps on more CTAs (10k nodes: 79 x 128 instead of 105 x 96)
   // (the incremental kernel only: the general kernel keeps one node per thread at its 128-thread blocks)
   const int R0 = s->dims.n_dims, K0 = s->dims.n_kdims;
   const bool samp_ok0 = s->dc.to_find == 0 || (s->world <= 1 && !s->dc.soft_active && (s->all_pure || !s->dc.enable_ecache));
