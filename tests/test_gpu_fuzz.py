@@ -51,18 +51,24 @@ def test_random_clusters_match_oracle(block, oracle_engine):
     assert checked >= 30
 
 
-@pytest.mark.parametrize("block", range(4))
+@pytest.mark.parametrize("block", range(6))
 def test_random_preempt_reclaim_match_oracle(block, oracle_engine):
     """The preempt and reclaim actions (alone, after allocate, in either order) on random clusters of running and pending
-    pods (tools/fuzz_evict.py): every statement (evictions, pipelines, commit / discard) identical to the oracle's."""
+    pods (tools/fuzz_evict.py): every statement (evictions, pipelines, commit / discard) identical to the oracle's.
+    Blocks 0-3: small clusters of 1-6 nodes; blocks 4-5: wide clusters (up to 3 000 mostly identical nodes, nodes running
+    more than 16 pods, R > 8)."""
     from volcano_b200 import engine
     engine.init(0)
     spec = importlib.util.spec_from_file_location("fuzz_evict", os.path.join(ROOT, "tools", "fuzz_evict.py"))
     gen = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(gen)
+    if block < 4:
+        seeds, make_case, need = range(3000 + 60 * block, 3000 + 60 * (block + 1)), gen.make_case, 40
+    else:
+        seeds, make_case, need = range(5000 + 20 * (block - 4), 5000 + 20 * (block - 3)), gen.make_wide_case, 20
     checked = ops = 0
-    for seed in range(3000 + 60 * block, 3000 + 60 * (block + 1)):
-        tc, tiers, actions = gen.make_case(seed)
+    for seed in seeds:
+        tc, tiers, actions = make_case(seed)
         snap = tc.RegisterSession(tiers, actions=actions)
         if snap.T == 0 or snap.N == 0 or snap.B > 0:
             continue
@@ -70,4 +76,4 @@ def test_random_preempt_reclaim_match_oracle(block, oracle_engine):
         res = engine.gpu_engine(snap)
         ops += gen.compare(res, ref, seed)
         checked += 1
-    assert checked >= 40 and ops >= 1
+    assert checked >= need and ops >= 1

@@ -507,6 +507,65 @@ def test_cfg5_cycle_vs_oracle(gpu, oracle_engine):
     assert (ref.preempt.decisions["kind"] == 2).sum() + (ref.reclaim.decisions["kind"] == 2).sum() > 10
 
 
+def test_cfg5_cycle_10k_vs_oracle(gpu, oracle_engine):
+    """BASELINE configs[4] at its full node count (10 000 nodes near capacity, 8 queues) with ~1 500 pending tasks: each
+    thread of the cached pick kernel owns ~10 nodes, so every hand-out repairs a lane's list by rescanning several nodes."""
+    from volcano_b200.synth import make_cfg5
+    snap = make_cfg5(seed=77, n_nodes=10_000, n_pending=1500, n_queues=8, utilisation=0.9)
+    res = gpu.gpu_engine(snap)
+    ref = oracle_engine(snap, threads=_host_threads())
+    _assert_same(res, ref)
+    _assert_same_evict(res.preempt, ref.preempt)
+    _assert_same_evict(res.reclaim, ref.reclaim)
+    assert (ref.preempt.decisions["kind"] == 2).sum() > 100 and (ref.reclaim.decisions["kind"] == 2).sum() > 100
+
+
+def test_evict_past_the_pick_cache_vs_oracle(gpu, oracle_engine):
+    """More than 25 600 nodes: the candidates' keys no longer fit in shared memory and production hands out candidates
+    with k_evict_pick_big. A small pending set keeps the oracle quick."""
+    from volcano_b200.synth import make_cfg5
+    snap = make_cfg5(seed=5, n_nodes=26_000, n_pending=200, n_queues=8, utilisation=0.6)
+    assert snap.N * 8 > 200 * 1024
+    res = gpu.gpu_engine(snap)
+    ref = oracle_engine(snap, threads=_host_threads())
+    _assert_same(res, ref)
+    _assert_same_evict(res.preempt, ref.preempt)
+    _assert_same_evict(res.reclaim, ref.reclaim)
+    assert (ref.preempt.decisions["kind"] == 2).sum() + (ref.reclaim.decisions["kind"] == 2).sum() > 10
+
+
+def _victims_cluster(n_victims):
+    """One node full of single-core pods of a low-priority job, and a starving high-priority job of the same queue whose
+    one pod needs n_victims of those cores back."""
+    from volcano_b200.api import BuildNode, BuildPod, BuildPodGroup, BuildQueue, BuildResourceList
+    from volcano_b200.snapshot import PluginOption
+    from volcano_b200.uthelper import TestCommonStruct
+    cores = n_victims + 1
+    node = BuildNode("n0", BuildResourceList(str(cores), f"{cores}Gi", ("pods", str(cores + 10))))
+    low = BuildPodGroup("low", "ns", "q", 1, None, "Running")
+    high = BuildPodGroup("high", "ns", "q", 1, None, "Inqueue")
+    low.priority, high.priority = 1, 100
+    pods = [BuildPod("ns", f"low-{k}", "n0", "Running", BuildResourceList("1", "1Gi"), "low", {}) for k in range(cores)]
+    pods.append(BuildPod("ns", "high-0", "", "Pending", BuildResourceList(str(n_victims), "1Gi"), "high", {}))
+    tc = TestCommonStruct(Name=f"victims{n_victims}", Nodes=[node], Pods=pods, PodGroups=[low, high], Queues=[BuildQueue("q", 1, None)])
+    tiers = [[PluginOption.defaults("priority"), PluginOption.defaults("gang"), PluginOption.defaults("conformance")]]
+    return tc.RegisterSession(tiers, actions=("preempt",))
+
+
+def test_evict_max_victims(gpu, oracle_engine):
+    """EV_MAX_VICTIMS: a preemptor that needs exactly 256 victims on one node matches the oracle; one that needs 257 is
+    refused with VC_EUNSUPPORTED instead of overrunning the apply command."""
+    snap = _victims_cluster(256)
+    res, ref = gpu.gpu_engine(snap), oracle_engine(snap)
+    _assert_same_evict(res.preempt, ref.preempt)
+    assert (ref.preempt.decisions["kind"] == 2).sum() == 256 and (ref.preempt.decisions["kind"] == 1).sum() == 1
+    snap = _victims_cluster(257)
+    assert (oracle_engine(snap).preempt.decisions["kind"] == 2).sum() == 257
+    with pytest.raises(gpu.VcError) as ei:
+        gpu.gpu_engine(snap)
+    assert ei.value.code == abi_mod().VC_EUNSUPPORTED
+
+
 def test_nominated_node_vs_oracle(gpu, oracle_engine):
     """Pod.Status.NominatedNodeName (actions/allocate/allocate.go:624-634): the nominated node is tried first, alone; parity
     with the oracle in the full-evaluation mode and with feasible-node sampling (where the one-node PredicateNodes call

@@ -81,6 +81,56 @@ def make_case(seed):
             p.priority_class_name = "system-cluster-critical"
             p.uid = ""
             p.__post_init__()
+    tiers, actions = _plugins_and_actions(rnd)
+    tc = TestCommonStruct(Name=f"evict-fuzz{seed}", Nodes=nodes, Pods=pods, PodGroups=pgs, Queues=queues)
+    return tc, tiers, actions
+
+
+def make_wide_case(seed):
+    """Wide clusters: 40-3 000 mostly identical nodes (equal scores: ties across every warp of the pick kernel, and idle
+    nodes that pass the node filter but offer no victim, so a preemptor walks past many candidates), a few nodes running
+    more than 16 pods, and 9 or more resource names (R > 8)."""
+    rnd = random.Random(seed * 7919 + 11)
+    n_nodes = rnd.randint(40, 3000)
+    scalars = [f"example.com/s{i}" for i in range(rnd.randint(7, 9))]
+    base = BuildResourceList("16", "32G", ("pods", "110"), *[(s, "4") for s in scalars])
+    odd = BuildResourceList("8", "32G", ("pods", "110"), *[(s, "4") for s in scalars])
+    nodes = [BuildNode(f"n{i:04d}", odd if rnd.random() < 0.05 else base) for i in range(n_nodes)]
+    queues = [BuildQueue(f"q{q}", rnd.randint(1, 4), None) for q in range(rnd.randint(2, 3))]
+    # hot nodes: more than 16 running pods each, anywhere in the node list (often near its end)
+    hot = sorted({rnd.choice([rnd.randrange(n_nodes), n_nodes - 1 - rnd.randrange(min(n_nodes, 64))])
+                  for _ in range(rnd.randint(1, 3))})
+    pgs, pods = [], []
+    small = BuildResourceList("500m", "512M", *[(s, "0") for s in scalars[:2]])
+    for j, node in enumerate(hot):  # one running job per hot node, 24-30 pods: 1-4 of its 16 cores left
+        q = rnd.randrange(len(queues))
+        n_run = rnd.randint(24, 30)
+        pgs.append(BuildPodGroup(f"hot{j}", "ns", f"q{q}", rnd.choice([1, n_run // 2, n_run]), None, "Running"))
+        pgs[-1].priority = rnd.choice([0, 10])
+        for k in range(n_run):
+            labels = {"volcano.sh/preemptable": "true"} if rnd.random() < 0.8 else {}
+            pods.append(BuildPod("ns", f"hot{j}-{k}", nodes[node].name, "Running", small, f"hot{j}", labels))
+    n_spread = rnd.randint(0, min(300, n_nodes))  # single running pods on random nodes
+    if n_spread:
+        q = rnd.randrange(len(queues))
+        pgs.append(BuildPodGroup("spread", "ns", f"q{q}", 1, None, "Running"))
+        for k in range(n_spread):
+            pods.append(BuildPod("ns", f"spread-{k}", rnd.choice(nodes).name, "Running",
+                                 BuildResourceList("2", "2G", (rnd.choice(scalars), "1")), "spread", {}))
+    for j in range(rnd.randint(1, 3)):  # starving jobs: their pods need the whole of some scalar a hot node holds
+        q = rnd.randrange(len(queues))
+        n_pend = rnd.randint(1, 4)
+        pgs.append(BuildPodGroup(f"pend{j}", "ns", f"q{q}", n_pend, None, rnd.choice(["Inqueue", "Running"])))
+        pgs[-1].priority = rnd.choice([10, 1000])
+        req = BuildResourceList(rnd.choice(["4", "15"]), "4G", *[(s, "1") for s in rnd.sample(scalars, rnd.randint(1, 4))])
+        for k in range(n_pend):
+            pods.append(BuildPod("ns", f"pend{j}-{k}", "", "Pending", req, f"pend{j}", {}))
+    tiers, actions = _plugins_and_actions(rnd)
+    tc = TestCommonStruct(Name=f"evict-wide{seed}", Nodes=nodes, Pods=pods, PodGroups=pgs, Queues=queues)
+    return tc, tiers, tuple(a for a in actions if a != "allocate") or ("preempt",)  # allocate would fill the idle nodes
+
+
+def _plugins_and_actions(rnd):
     voters = [n for n in ("conformance", "gang", "priority", "drf", "proportion") if rnd.random() < 0.75]
     scorers = [n for n in ("predicates", "nodeorder", "binpack") if rnd.random() < 0.5]
     chosen = voters + scorers
@@ -96,8 +146,7 @@ def make_case(seed):
         actions = ("enqueue",) + actions
     if rnd.random() < 0.2 and "preempt" in actions and "reclaim" in actions:
         actions = tuple(a for a in actions if a not in ("preempt", "reclaim")) + ("reclaim", "preempt")
-    tc = TestCommonStruct(Name=f"evict-fuzz{seed}", Nodes=nodes, Pods=pods, PodGroups=pgs, Queues=queues)
-    return tc, tiers, actions
+    return tiers, actions
 
 
 def compare(res, ref, seed):

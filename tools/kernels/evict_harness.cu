@@ -1,0 +1,263 @@
+// evict_harness.cu — test-only launchers for the preempt / reclaim kernels of volcano_b200/csrc/vc_evict.cuh.
+//
+// Every launcher takes host arrays and sizes, checks them on the host (sizes within the kernel's limits, every index in
+// range) and returns EH_EINVAL without launching when they are not; otherwise it stages the data on the device, builds
+// EvictParams / EvictTask / DevConf as vcalloc.cu does, launches with the production geometry and copies the results back.
+// The pick hand-outs and the apply command live in mapped pinned memory, as in production.
+#include <cstring>
+#include <vector>
+
+#include "../../volcano_b200/csrc/vc_evict.cuh"
+
+#define EH_OK 0
+#define EH_EINVAL (-1)
+#define EH_ECUDA (-3)
+
+#define EH_TRY(x)                                  \
+  do {                                             \
+    if ((x) != cudaSuccess) return EH_ECUDA;       \
+  } while (0)
+
+namespace {
+
+template <class T>
+struct DevBuf {  // device copy of a host array (nullptr for an empty one)
+  T *d = nullptr;
+  ~DevBuf() { if (d) cudaFree(d); }
+  cudaError_t put(const T *h, size_t n) {
+    if (n == 0) return cudaSuccess;
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&d), n * sizeof(T));
+    if (e != cudaSuccess) return e;
+    return h ? cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice) : cudaMemset(d, 0, n * sizeof(T));
+  }
+  cudaError_t get(T *h, size_t n) const { return n ? cudaMemcpy(h, d, n * sizeof(T), cudaMemcpyDeviceToHost) : cudaSuccess; }
+};
+
+struct Mapped {  // mapped pinned int32 words
+  int32_t *h = nullptr, *d = nullptr;
+  ~Mapped() { if (h) cudaFreeHost(h); }
+  cudaError_t alloc(size_t n) {
+    cudaError_t e = cudaHostAlloc(reinterpret_cast<void **>(&h), n * 4, cudaHostAllocMapped);
+    if (e != cudaSuccess) return e;
+    return cudaHostGetDevicePointer(reinterpret_cast<void **>(&d), h, 0);
+  }
+};
+
+}  // namespace
+
+// ---- k_evict_pick / k_evict_pick_big --------------------------------------------------------------------------------
+// A pick state holds the candidate flags and keys of N nodes on the device; each eh_pick_launch is one production launch
+// on that state (cand 1 -> 2 for the nodes handed out), so a test drains it the way the host control loop does.
+struct EhPick {
+  int N = 0;
+  DevBuf<uint8_t> cand;
+  DevBuf<unsigned long long> key;
+  Mapped pick;  // [0, EV_PICK_K) hand-outs, [EV_PICK_K] sequence word
+};
+
+extern "C" int eh_pick_smem_max_nodes() { return 200 * 1024 / 8; }  // vcalloc.cu's switch to k_evict_pick_big
+
+extern "C" int eh_pick_open(int N, const uint8_t *cand, const unsigned long long *key, EhPick **out) {
+  if (!out || N < 0 || (N > 0 && (!cand || !key))) return EH_EINVAL;
+  for (int n = 0; n < N; ++n)
+    if (cand[n] > 2) return EH_EINVAL;
+  EhPick *s = new EhPick();
+  s->N = N;
+  if (s->cand.put(cand, N) != cudaSuccess || s->key.put(key, N) != cudaSuccess || s->pick.alloc(EV_PICK_K + 1) != cudaSuccess) {
+    delete s;
+    return EH_ECUDA;
+  }
+  *out = s;
+  return EH_OK;
+}
+
+extern "C" void eh_pick_close(EhPick *s) { delete s; }
+
+// big = 0: k_evict_pick with N * 8 bytes of dynamic shared memory (N <= eh_pick_smem_max_nodes()); 1: k_evict_pick_big.
+// words[0..EV_PICK_K] receive the mapped buffer after the launch (hand-outs, then the sequence word), which is set to
+// ~seq before it; cand_out (N bytes, may be null) receives the flags.
+extern "C" int eh_pick_launch(EhPick *s, int big, int mode, int seq, int32_t *words, uint8_t *cand_out) {
+  if (!s || !words || (big != 0 && big != 1) || mode < EV_MODE_PREEMPT_INTER || mode > EV_MODE_RECLAIM) return EH_EINVAL;
+  const size_t smem = (size_t)s->N * 8;
+  if (!big && s->N > eh_pick_smem_max_nodes()) return EH_EINVAL;
+  EvictParams p;
+  std::memset(&p, 0, sizeof p);
+  p.d.N = s->N;
+  p.cand = s->cand.d;
+  p.key = s->key.d;
+  p.pick_node = s->pick.d;
+  for (int i = 0; i < EV_PICK_K; ++i) s->pick.h[i] = -7;
+  s->pick.h[EV_PICK_K] = ~seq;
+  if (!big) {
+    if (smem > 48 * 1024) EH_TRY(cudaFuncSetAttribute(k_evict_pick, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_evict_pick<<<1, 1024, smem>>>(p, mode, seq);
+  } else {
+    k_evict_pick_big<<<1, 1024, 0>>>(p, mode, seq);
+  }
+  EH_TRY(cudaGetLastError());
+  EH_TRY(cudaDeviceSynchronize());
+  for (int i = 0; i <= EV_PICK_K; ++i) words[i] = reinterpret_cast<volatile int32_t *>(s->pick.h)[i];
+  if (cand_out) EH_TRY(s->cand.get(cand_out, s->N));
+  return EH_OK;
+}
+
+// ---- k_evict_rank ---------------------------------------------------------------------------------------------------
+// One preemptor against N nodes. Only the victim-voting plugins may be enabled (no VC_EN_NODE_ORDER: the harness carries
+// no scoring rows), so every candidate's key is ev_score_key(+0.0). Class 0 is the preemptor's; cstat is its row [N].
+struct EhRankArgs {
+  int N, R, RT, J, Q, pods_dim, exact_sums;
+  int n_plugins;
+  const int32_t *plugin, *tier;
+  const uint32_t *enabled;
+  const double *idle, *rel, *pip;  // [R][N]
+  const uint32_t *cstat;           // [N]
+  const int32_t *rt_off, *rt_idx;  // [N+1], [RT]
+  const double *rt_req;            // [R][RT]
+  const uint32_t *rt_flags;        // [RT]
+  const int32_t *rt_job, *rt_prio; // [RT]
+  const uint8_t *rt_evicted;       // [RT]
+  const int32_t *j_queue, *j_prio, *j_min, *j_ready;  // [J]
+  const uint32_t *q_flags;         // [Q]
+  const uint8_t *q_over;           // [Q]
+  // the preemptor
+  int mode, job, queue, job_prio, task_prio;
+  const double *req;  // [R]
+  uint32_t has;
+  int quota_on, quota_open;
+  uint32_t qalloc_has, qdes_has;
+  const double *qalloc, *qdes;  // [R]
+  // results
+  uint8_t *cand;            // [N]
+  unsigned long long *key;  // [N]
+};
+
+extern "C" int eh_rank(const EhRankArgs *a) {
+  if (!a) return EH_EINVAL;
+  const int N = a->N, R = a->R, RT = a->RT, J = a->J, Q = a->Q;
+  if (N < 0 || R < 2 || R > VC_MAX_DIMS || RT < 0 || J < 0 || Q < 0 || a->pods_dim < -1 || a->pods_dim >= R) return EH_EINVAL;
+  if (a->n_plugins < 0 || a->n_plugins > VC_MAX_PLUGINS) return EH_EINVAL;
+  if (a->mode < EV_MODE_PREEMPT_INTER || a->mode > EV_MODE_RECLAIM || a->job < -1 || a->job >= J || a->queue < -1 || a->queue >= Q)
+    return EH_EINVAL;
+  if (!a->req || (a->quota_on && (!a->qalloc || !a->qdes)) || !a->cand || !a->key) return EH_EINVAL;
+  if (N > 0 && (!a->idle || !a->rel || !a->pip || !a->cstat || !a->rt_off)) return EH_EINVAL;
+  if (RT > 0 && (!a->rt_idx || !a->rt_req || !a->rt_flags || !a->rt_job || !a->rt_prio || !a->rt_evicted)) return EH_EINVAL;
+  if (J > 0 && (!a->j_queue || !a->j_prio || !a->j_min || !a->j_ready)) return EH_EINVAL;
+  if (Q > 0 && (!a->q_flags || !a->q_over)) return EH_EINVAL;
+  DevConf c;
+  std::memset(&c, 0, sizeof c);
+  c.n_plugins = a->n_plugins;
+  for (int i = 0; i < a->n_plugins; ++i) {
+    if (a->plugin[i] < 0 || (i > 0 && a->tier[i] < a->tier[i - 1]) || (a->enabled[i] & VC_EN_NODE_ORDER)) return EH_EINVAL;
+    c.plugin[i] = a->plugin[i]; c.tier[i] = a->tier[i]; c.enabled[i] = a->enabled[i];
+  }
+  // node.Tasks: CSR over the nodes, every entry a running task, every task's job / queue in range
+  if (N > 0 && (a->rt_off[0] != 0 || a->rt_off[N] != RT)) return EH_EINVAL;
+  for (int n = 0; n < N; ++n)
+    if (a->rt_off[n + 1] < a->rt_off[n]) return EH_EINVAL;
+  for (int k = 0; k < RT; ++k) {
+    if (a->rt_idx[k] < 0 || a->rt_idx[k] >= RT) return EH_EINVAL;
+    if (a->rt_job[k] < -1 || a->rt_job[k] >= J) return EH_EINVAL;
+  }
+  for (int j = 0; j < J; ++j)
+    if (a->j_queue[j] < -1 || a->j_queue[j] >= Q) return EH_EINVAL;
+
+  DevBuf<double> idle, rel, pip, rt_req;
+  DevBuf<uint32_t> cstat, rt_flags, q_flags;
+  DevBuf<int32_t> rt_off, rt_idx, rt_job, rt_prio, j_queue, j_prio, j_min, j_ready;
+  DevBuf<uint8_t> rt_ev, q_over, cand;
+  DevBuf<unsigned long long> key;
+  const size_t RN = (size_t)R * N;
+  EH_TRY(idle.put(a->idle, RN)); EH_TRY(rel.put(a->rel, RN)); EH_TRY(pip.put(a->pip, RN));
+  EH_TRY(cstat.put(a->cstat, N)); EH_TRY(rt_off.put(a->rt_off, N > 0 ? N + 1 : 0));
+  EH_TRY(rt_idx.put(a->rt_idx, RT)); EH_TRY(rt_req.put(a->rt_req, (size_t)R * RT)); EH_TRY(rt_flags.put(a->rt_flags, RT));
+  EH_TRY(rt_job.put(a->rt_job, RT)); EH_TRY(rt_prio.put(a->rt_prio, RT)); EH_TRY(rt_ev.put(a->rt_evicted, RT));
+  EH_TRY(j_queue.put(a->j_queue, J)); EH_TRY(j_prio.put(a->j_prio, J)); EH_TRY(j_min.put(a->j_min, J));
+  EH_TRY(j_ready.put(a->j_ready, J)); EH_TRY(q_flags.put(a->q_flags, Q)); EH_TRY(q_over.put(a->q_over, Q));
+  EH_TRY(cand.put(nullptr, N)); EH_TRY(key.put(nullptr, N));
+
+  EvictParams p;
+  std::memset(&p, 0, sizeof p);
+  p.d.N = N; p.d.R = R; p.d.K = 0; p.d.C = 1; p.d.J = J; p.d.Q = Q; p.d.pods_dim = a->pods_dim;
+  p.c = c;
+  p.idle = idle.d; p.rel = rel.d; p.pip = pip.d; p.cstat = cstat.d;
+  p.rt_off = rt_off.d; p.rt_idx = rt_idx.d; p.rt_req = rt_req.d; p.rt_flags = rt_flags.d; p.rt_job = rt_job.d;
+  p.rt_prio = rt_prio.d; p.rt_evicted = rt_ev.d; p.j_queue = j_queue.d; p.j_prio = j_prio.d; p.j_min = j_min.d;
+  p.j_ready = j_ready.d; p.q_flags = q_flags.d; p.q_over = q_over.d;
+  p.exact_sums = a->exact_sums ? 1 : 0;
+  p.RT = RT;
+  p.key = key.d; p.cand = cand.d;
+  EvictTask t;
+  std::memset(&t, 0, sizeof t);
+  for (int d = 0; d < R; ++d) t.rec.req[d] = a->req[d];
+  t.rec.has = a->has; t.rec.klass = 0;
+  t.klass = 0; t.job = a->job; t.queue = a->queue; t.mode = a->mode; t.job_prio = a->job_prio; t.task_prio = a->task_prio;
+  t.quota_on = a->quota_on ? 1 : 0; t.quota_open = a->quota_open ? 1 : 0;
+  t.qalloc_has = a->qalloc_has; t.qdes_has = a->qdes_has;
+  if (a->quota_on)
+    for (int d = 0; d < R; ++d) { t.qalloc[d] = a->qalloc[d]; t.qdes[d] = a->qdes[d]; }
+  if (N > 0) {  // the instance vcalloc.cu picks for R
+    if (R <= 8) k_evict_rank<16, 8><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);
+    else k_evict_rank<16, VC_MAX_DIMS><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);
+    EH_TRY(cudaGetLastError());
+  }
+  EH_TRY(cudaDeviceSynchronize());
+  EH_TRY(cand.get(a->cand, N));
+  EH_TRY(key.get(a->key, N));
+  return EH_OK;
+}
+
+// ---- k_evict_apply --------------------------------------------------------------------------------------------------
+// Statement.Evict of the victims + Statement.Pipeline of the preemptor on one node (undo = 0), or the inverse (undo = 1).
+// The rows are updated in place: rel, pip [R][N]; kreq [K][N]; knz [2][N]; pod_count [N]; rt_evicted [RT].
+struct EhApplyArgs {
+  int N, R, K, RT, has_predicates;
+  double *rel, *pip, *kreq, *knz;
+  int32_t *pod_count;
+  uint8_t *rt_evicted;
+  const double *rt_req, *rt_kreq, *rt_knz;  // [R][RT], [K][RT], [2][RT]
+  const double *req, *kreq_t, *knz_t;       // the preemptor: [R], [K], [2]
+  int node, n_victims;
+  const int32_t *victims;
+  int undo;
+};
+
+extern "C" int eh_apply(const EhApplyArgs *a) {
+  if (!a) return EH_EINVAL;
+  const int N = a->N, R = a->R, K = a->K, RT = a->RT;
+  if (N < 1 || R < 1 || R > VC_MAX_DIMS || K < 0 || K > VC_MAX_KDIMS || RT < 0) return EH_EINVAL;
+  if (a->node < 0 || a->node >= N || a->n_victims < 0 || a->n_victims > EV_MAX_VICTIMS) return EH_EINVAL;
+  if (!a->rel || !a->pip || !a->knz || !a->pod_count || !a->req || !a->knz_t || (K > 0 && (!a->kreq || !a->kreq_t))) return EH_EINVAL;
+  if (RT > 0 && (!a->rt_evicted || !a->rt_req || !a->rt_knz || (K > 0 && !a->rt_kreq))) return EH_EINVAL;
+  if (a->n_victims > 0 && !a->victims) return EH_EINVAL;
+  for (int i = 0; i < a->n_victims; ++i)
+    if (a->victims[i] < 0 || a->victims[i] >= RT) return EH_EINVAL;
+  DevBuf<double> rel, pip, kreq, knz, rt_req, rt_kreq, rt_knz;
+  DevBuf<int32_t> pod_count;
+  DevBuf<uint8_t> rt_ev;
+  EH_TRY(rel.put(a->rel, (size_t)R * N)); EH_TRY(pip.put(a->pip, (size_t)R * N)); EH_TRY(kreq.put(a->kreq, (size_t)K * N));
+  EH_TRY(knz.put(a->knz, (size_t)2 * N)); EH_TRY(pod_count.put(a->pod_count, N)); EH_TRY(rt_ev.put(a->rt_evicted, RT));
+  EH_TRY(rt_req.put(a->rt_req, (size_t)R * RT)); EH_TRY(rt_kreq.put(a->rt_kreq, (size_t)K * RT));
+  EH_TRY(rt_knz.put(a->rt_knz, (size_t)2 * RT));
+  Mapped cmd;
+  EH_TRY(cmd.alloc(2 + EV_MAX_VICTIMS));
+  cmd.h[0] = a->node; cmd.h[1] = a->n_victims;
+  for (int i = 0; i < a->n_victims; ++i) cmd.h[2 + i] = a->victims[i];
+  EvictParams p;
+  std::memset(&p, 0, sizeof p);
+  p.d.N = N; p.d.R = R; p.d.K = K;
+  p.c.has_predicates = a->has_predicates ? 1 : 0;
+  p.rel = rel.d; p.pip = pip.d; p.kreq = kreq.d; p.knz = knz.d; p.pod_count = pod_count.d; p.rt_evicted = rt_ev.d;
+  p.rt_req = rt_req.d; p.rt_kreq = rt_kreq.d; p.rt_knz = rt_knz.d; p.RT = RT;
+  p.cmd = cmd.d;
+  EvictTask t;
+  std::memset(&t, 0, sizeof t);
+  for (int d = 0; d < R; ++d) t.rec.req[d] = a->req[d];
+  for (int k = 0; k < K; ++k) t.rec.kreq[k] = a->kreq_t[k];
+  for (int k = 0; k < 2; ++k) t.rec.knz[k] = a->knz_t[k];
+  k_evict_apply<<<1, 64>>>(p, t, a->undo ? 1 : 0);
+  EH_TRY(cudaGetLastError());
+  EH_TRY(cudaDeviceSynchronize());
+  EH_TRY(rel.get(a->rel, (size_t)R * N)); EH_TRY(pip.get(a->pip, (size_t)R * N)); EH_TRY(kreq.get(a->kreq, (size_t)K * N));
+  EH_TRY(knz.get(a->knz, (size_t)2 * N)); EH_TRY(pod_count.get(a->pod_count, N)); EH_TRY(rt_ev.get(a->rt_evicted, RT));
+  return EH_OK;
+}

@@ -216,13 +216,11 @@ __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) 
 // one block: the next EV_PICK_K candidates in the action's node order (preempt: score descending, lowest index first
 // among equals; reclaim: index ascending); the nodes handed out are marked tried. Tournament with incremental repair:
 // every thread keeps the best of its own nodes in registers, every warp its best in shared memory; handing out a node
-// makes ONE thread rescan its nodes and ONE warp refold, the other 31 entries stay.
-// `cached` != 0: the launch carries N * 8 bytes of dynamic shared memory and the keys of the live candidates are staged there
-// once (0 = not a candidate), so that repairs read shared memory instead of global memory.
-extern __shared__ unsigned long long ev_pick_cache[];
+// makes ONE thread rescan its nodes and ONE warp refold, the other 31 entries stay. Used when the keys do not fit in shared
+// memory (k_evict_pick below): repairs read the candidate flags and keys from global memory.
 // The last store of the launch is `seq` into pick_node[EV_PICK_K] (system scope): the host polls that word of the mapped
 // buffer instead of paying a stream synchronisation per hand-out.
-__global__ void k_evict_pick_big(EvictParams p, int mode, int cached, int seq) {
+__global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
   __shared__ unsigned long long s_key[32];
   __shared__ int s_node[32];
   __shared__ int s_best;
@@ -230,11 +228,6 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int cached, int seq) {
                                      // per iteration sits on the critical path of the block-wide barriers)
   const int N = p.d.N;
   if (threadIdx.x < EV_PICK_K) s_pick[threadIdx.x] = -1;
-  if (cached) {  // key + 1 (the top bit of a score key is never clear with all others set), 0 = not a candidate
-    for (int n = threadIdx.x; n < N; n += blockDim.x)
-      ev_pick_cache[n] = p.cand[n] == 1 ? (mode == EV_MODE_RECLAIM ? 1ull : p.key[n] + 1ull) : 0ull;
-    __syncthreads();
-  }
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
   auto better_kn = [](unsigned long long ka, int na, unsigned long long kb, int nb) {
     return na >= 0 && (nb < 0 || ka > kb || (ka == kb && na < nb));
@@ -243,14 +236,6 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int cached, int seq) {
   int bn = -1;
   auto rescan = [&](int skip) {
     bk = 0ull; bn = -1;
-    if (cached) {
-      for (int n = threadIdx.x; n < N; n += blockDim.x) {
-        const unsigned long long k = ev_pick_cache[n];
-        if (n == skip || k == 0ull) continue;
-        if (bn < 0 || k > bk) { bk = k; bn = n; }
-      }
-      return;
-    }
     for (int n = threadIdx.x; n < N; n += blockDim.x) {
       if (n == skip || p.cand[n] != 1) continue;
       const unsigned long long k = mode == EV_MODE_RECLAIM ? 0ull : p.key[n];
@@ -281,7 +266,7 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int cached, int seq) {
       }
       if (lane == 0) {
         s_pick[it] = gn;
-        if (gn >= 0) { p.cand[gn] = 2; if (cached) ev_pick_cache[gn] = 0ull; }
+        if (gn >= 0) p.cand[gn] = 2;
         s_best = gn;
       }
     }
@@ -311,6 +296,7 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int cached, int seq) {
 // keeps the best of its ~N/1024 nodes in registers, the winner rescans its shared-memory entries) give the warp's first
 // EV_PICK_K candidates in order. Phase 2, one warp: a 32-way merge of those sorted lists. Same order as the sequential
 // tournament: key descending, node ascending.
+extern __shared__ unsigned long long ev_pick_cache[];
 __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, int seq) {
   __shared__ unsigned long long l_key[32][EV_PICK_K];
   __shared__ int l_node[32][EV_PICK_K];
@@ -383,15 +369,24 @@ __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, in
 
 // Statement.Evict for every victim (node.UpdateTask: Releasing += Resreq; predicates DeallocateFunc: RemovePod), then
 // Statement.Pipeline of the preemptor (Pipelined += Resreq; predicates AllocateFunc: AddPod) on node cmd[0]
-// `undo` != 0: the inverse (Statement.Discard: UnPipeline, then unevict in reverse order; the sums are integer-valued
-// doubles, so the order of the subtractions does not show)
+// `undo` != 0: the inverse in Statement.Discard's order (UnPipeline, then unevict the victims in reverse order), so that
+// with non-integer requests the rows come back exactly as the reference's discard leaves them.
 __global__ void k_evict_apply(EvictParams p, EvictTask t, int undo) {
   const int n = p.cmd[0], nv = p.cmd[1];
   const int N = p.d.N, R = p.d.R, K = p.d.K;
   const int d = threadIdx.x;
   const double sg = undo ? -1.0 : 1.0;
-  for (int k = 0; k < nv; ++k) {
-    const int r = p.cmd[2 + k];
+  auto pipeline = [&]() {
+    if (d < R) p.pip[(size_t)d * N + n] += sg * t.rec.req[d];
+    if (p.c.has_predicates) {
+      if (d >= 32 && d < 32 + K) p.kreq[(size_t)(d - 32) * N + n] += sg * t.rec.kreq[d - 32];
+      if (d >= 48 && d < 50) p.knz[(size_t)(d - 48) * N + n] += sg * t.rec.knz[d - 48];
+      if (d == 62) p.pod_count[n] += undo ? nv - 1 : 1 - nv;
+    }
+  };
+  if (undo) pipeline();
+  for (int i = 0; i < nv; ++i) {
+    const int r = p.cmd[2 + (undo ? nv - 1 - i : i)];
     if (d < R) p.rel[(size_t)d * N + n] += sg * p.rt_req[(size_t)d * p.RT + r];
     if (p.c.has_predicates) {
       if (d >= 32 && d < 32 + K) p.kreq[(size_t)(d - 32) * N + n] -= sg * p.rt_kreq[(size_t)(d - 32) * p.RT + r];
@@ -399,10 +394,5 @@ __global__ void k_evict_apply(EvictParams p, EvictTask t, int undo) {
     }
     if (d == 63) p.rt_evicted[r] = undo ? 0 : 1;
   }
-  if (d < R) p.pip[(size_t)d * N + n] += sg * t.rec.req[d];
-  if (p.c.has_predicates) {
-    if (d >= 32 && d < 32 + K) p.kreq[(size_t)(d - 32) * N + n] += sg * t.rec.kreq[d - 32];
-    if (d >= 48 && d < 50) p.knz[(size_t)(d - 48) * N + n] += sg * t.rec.knz[d - 48];
-    if (d == 62) p.pod_count[n] += undo ? nv - 1 : 1 - nv;
-  }
+  if (!undo) pipeline();
 }

@@ -1898,7 +1898,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   auto launch_pick = [&](int k, int mode) -> int {
     sets[k].seq += 1;
     if (pick_smem) k_evict_pick<<<1, 1024, pick_smem, s->stream>>>(with_set(k), mode, sets[k].seq);
-    else k_evict_pick_big<<<1, 1024, 0, s->stream>>>(with_set(k), mode, 0, sets[k].seq);
+    else k_evict_pick_big<<<1, 1024, 0, s->stream>>>(with_set(k), mode, sets[k].seq);
     launches++;
     CUDA_TRY(cudaGetLastError());
     return VC_OK;
