@@ -422,7 +422,8 @@ int vc_comm_attach(vc_snapshot *s, const void *handles);
 int vc_comm_prepare(vc_snapshot *s);
 
 /* Restrict the node axis of this process to [node_begin, node_end) for node-sharded
-   multi-GPU runs (SURVEY §8e); tasks/jobs/queues stay replicated. Default: all nodes. */
+   multi-GPU runs (SURVEY §8e); tasks/jobs/queues stay replicated. Default: all nodes.
+   A non-empty shard begins at a multiple of 64 (one mask word per shard); an empty one may begin anywhere. */
 int vc_snapshot_set_shard(vc_snapshot *s, int32_t node_begin, int32_t node_end);
 
 /* The allocate action on the uploaded snapshot: exact sequential greedy assignment. */

@@ -599,8 +599,10 @@ int vc_comm_prepare(vc_snapshot *s) {
 
 int vc_snapshot_set_shard(vc_snapshot *s, int32_t node_begin, int32_t node_end) {
   if (!s) return fail(VC_EINVAL, "null snapshot");
-  if (node_begin < 0 || node_end > s->dims.n_nodes || node_begin > node_end || (node_begin % 64) != 0)
-    return fail(VC_EINVAL, "shard [%d,%d) invalid (begin must be a multiple of 64)", node_begin, node_end);
+  // a mask word belongs to one shard, so a shard with nodes begins at a multiple of 64; an empty one owns no word and
+  // may begin anywhere (parallel.shard_bounds gives the ranks past the last node [N, N))
+  if (node_begin < 0 || node_end > s->dims.n_nodes || node_begin > node_end || ((node_begin % 64) != 0 && node_begin != node_end))
+    return fail(VC_EINVAL, "shard [%d,%d) invalid (a non-empty shard must begin at a multiple of 64)", node_begin, node_end);
   if (s->dd.node_begin == node_begin && s->dd.node_end == node_end) return VC_OK;  // unchanged: the dense-pass tables stay
   s->dd.node_begin = node_begin;
   s->dd.node_end = node_end;

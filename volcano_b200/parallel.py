@@ -74,6 +74,9 @@ def sharded_dense_best(eng, world: int, rank: int, device, materialize: bool = F
     ptr, count = eng.dense_stats_ptr()
     if count:
         reduce_group_stats(device_tensor(ptr, (count,), torch.int32, device))
+        # NCCL returns once the reduction is queued and orders only torch's current stream after it; the library's
+        # stream is non-blocking, so the scoring kernels of dense_finish would otherwise read the shard's local stats
+        torch.cuda.current_stream(device).synchronize()
     eng.dense_finish(materialize)
     ps, pn = eng.dense_best_ptrs()
     T = eng.snap.T
