@@ -252,6 +252,15 @@ func openCycle(ssn *framework.Session) bool {
 			return false
 		}
 	}
+	var hd *C.vc_hdrf // nil clears the table
+	if e.hdrf {
+		hd = &C.vc_hdrf{path_off: ptrI(e.hdPathOff), path_name: ptrI(e.hdPathName), n_weights: ptrI(e.hdNWeights),
+			weight: ptrF(e.hdWeight), job_request: ptrF(e.hdJobRequest)}
+	}
+	if rc := C.vc_snapshot_set_hdrf(cur.snap, hd); rc != 0 {
+		fail("hdrf table")
+		return false
+	}
 	bf := e.b.c()
 	if rc := C.vc_snapshot_set_backfill(cur.snap, C.int32_t(len(e.bfTasks)), &bf); rc != 0 {
 		fail("backfill list")

@@ -80,6 +80,11 @@ type session struct {
 	qUIDRank, qFlags, qCapHas, qGuarHas, qReqHas, qAllocHas []uint32
 	qCap, qGuar, qAlloc, qReq                       []float64
 	tFlags                                          []uint32
+	// vc_hdrf (drf's enableHierarchy): hdrf false = the option is off and the table is cleared
+	hdrf                    bool
+	hdPathOff, hdPathName   []int32
+	hdNWeights              []int32
+	hdWeight, hdJobRequest  []float64
 }
 
 type taskArrays struct {
@@ -714,7 +719,46 @@ func encodeSession(ssn *framework.Session, enqueueConfigured bool) *session {
 		n_classes: C.int32_t(C_), n_roles: C.int32_t(NR), n_dims: C.int32_t(R), n_kdims: C.int32_t(K),
 		label_words: C.int32_t(Wl), taint_words: C.int32_t(Wt), n_zones: C.int32_t(len(zones)), pods_dim: C.int32_t(e.podsDim)}
 	e.encodeConf(ssn.Tiers, enqueueConfigured)
+	if e.hdrf {
+		e.encodeHdrf(R)
+	}
 	return e
+}
+
+// encodeHdrf fills vc_hdrf: per queue the segments of QueueInfo.Hierarchy below the root as interned names, the number of
+// weight segments below the root and strconv.ParseFloat of each (the value it returns even with an error: the library
+// clamps it as buildHierarchy does, drf.go:458-500); per job JobInfo.TotalRequest. Tree construction and the refusal of
+// what the reference crashes on are the library's.
+func (e *session) encodeHdrf(R int) {
+	Q, J := len(e.queues), len(e.jobs)
+	names := map[string]int32{}
+	e.hdPathOff = make([]int32, Q+1)
+	e.hdNWeights = make([]int32, Q)
+	e.hdPathName, e.hdWeight = nil, nil
+	for qi, q := range e.queues {
+		paths := strings.Split(q.Hierarchy, "/")[1:]
+		weights := strings.Split(q.Weights, "/")[1:]
+		for i, seg := range paths {
+			id, ok := names[seg]
+			if !ok {
+				id = int32(len(names))
+				names[seg] = id
+			}
+			e.hdPathName = append(e.hdPathName, id)
+			w := 0.0
+			if i < len(weights) {
+				w, _ = strconv.ParseFloat(weights[i], 64)
+			}
+			e.hdWeight = append(e.hdWeight, w)
+		}
+		e.hdNWeights[qi] = int32(len(weights))
+		e.hdPathOff[qi+1] = int32(len(e.hdPathName))
+	}
+	e.hdJobRequest = make([]float64, R*J)
+	for ji, job := range e.jobs {
+		v, _ := e.vec(job.TotalRequest)
+		putCol(e.hdJobRequest, J, ji, v)
+	}
 }
 
 // the accounting rows of one node: the part vc_snapshot_update_nodes re-uploads when NodeInfo.Generation moved
@@ -768,7 +812,7 @@ func (e *session) encodeConf(tiers []conf.Tier, enqueueConfigured bool) {
 				id = C.VC_PLUGIN_OTHER
 			}
 			if p.Name == "drf" && on(p.EnabledHierarchy) { // hdrf: queue order from the hierarchy tree (drf/drf.go:147-156)
-				e.outOfScope = "drf with enableHierarchy"
+				e.hdrf = true
 			}
 			var en C.uint32_t
 			for flag, b := range map[C.uint32_t]*bool{C.VC_EN_JOB_ORDER: p.EnabledJobOrder, C.VC_EN_JOB_READY: p.EnabledJobReady,

@@ -279,6 +279,19 @@ typedef struct vc_hypernodes {
                                        (FindJobTaskNumOfHyperNode counts subJob.Tasks by NodeName) */
 } vc_hypernodes;
 
+/* ---- hierarchical drf (drf's enableHierarchy, plugins/drf/drf.go:45-184,458-560): the queue annotations
+   volcano.sh/hierarchy and volcano.sh/hierarchy-weights (QueueInfo.Hierarchy / Weights, api/queue_info.go:60-61), split
+   on "/" with the first segment (the root) dropped. The library builds the tree (first-creator weights, clamp to 1). ---- */
+typedef struct vc_hdrf {
+  const int32_t *path_off;  /* [Q+1] CSR over path_name: queue q names the segments [path_off[q], path_off[q+1]) */
+  const int32_t *path_name; /* interned segment names (equal ids = equal strings) */
+  const int32_t *n_weights; /* [Q] segments of the weights string after the first (len(split(Weights)) - 1) */
+  const double *weight;     /* laid out like path_name: strconv.ParseFloat of the weight segment at the same depth, the
+                               value ParseFloat returns even with an error (0 for a syntax error, +-Inf out of range);
+                               entries at depths >= n_weights[q] are ignored */
+  const double *job_request; /* [R][J] JobInfo.TotalRequest: Resreq summed over every task of the job, any status */
+} vc_hdrf;
+
 /* ---- node.Tasks: the pods that occupy nodes (api/node_info.go:88) — candidate victims of the preempt and
    reclaim actions. Their resources are already part of vc_nodes.{idle,used,...}; this table adds what victim
    selection reads per task. Index space of its own ("running task" r). ---- */
@@ -382,6 +395,17 @@ int vc_snapshot_update_nodes(vc_snapshot *s, int32_t n_dirty, const int32_t *nod
 /* Optional, before vc_snapshot_upload: the HyperNode tree of the session. Without it a configured
    network-topology-aware plugin scores against the cluster top hypernode only (no HyperNode CRs). */
 int vc_snapshot_set_topology(vc_snapshot *s, const vc_hypernodes *topo);
+
+/* Optional, before vc_snapshot_upload: the queue hierarchy of drf's enableHierarchy (passing it means the option is set;
+   NULL clears it). The table is copied; the tree is built at upload: children in first-insertion order with jobs inserted
+   in index order, so the node's creator (and its weight) is the first job's queue; a weight < 1 or unparsable becomes 1.
+   The allocate action then orders queues with hdrf's compareQueues in the tier chain of ssn.QueueOrderFn (when drf has
+   EnabledQueueOrder) on a Go heap re-evaluated at every Push / Pop, as util.PriorityQueue does, and backfill's pick
+   order uses the same chain on the state allocate left. VC_EINVAL at upload: drf not configured, a job outside ssn.Queues, a queue with jobs whose weights string
+   has fewer segments than its path (the reference crashes on both), non-integral task requests or job allocations.
+   vc_preempt_run / vc_reclaim_run return VC_EUNSUPPORTED with the table present (hdrf's reclaimFn is not built). Calling
+   this after vc_snapshot_upload requires a new upload. */
+int vc_snapshot_set_hdrf(vc_snapshot *s, const vc_hdrf *hdrf);
 
 /* Optional, before vc_snapshot_upload: the BestEffort pending tasks of the session (TaskInfo.BestEffort,
    api/job_info.go:188: Resreq empty but for pods:1; not scheduling-gated) — the tasks the backfill action

@@ -165,6 +165,35 @@ def make_case(seed, big=False):
     return tc, tiers, actions
 
 
+def make_hdrf_case(seed):
+    """The hdrf family: a make_case cluster with drf's enableHierarchy on and random volcano.sh/hierarchy annotations —
+    trees up to 4 levels below the root, nodes shared by several queues, root-level queues, weights that clamp to 1
+    ("0.5", "abc", "0") — and drf before or after proportion. Returns (case, tiers, actions, hierarchy, weights)."""
+    tc, tiers, actions = make_case(seed)
+    rnd = random.Random(seed * 15485863 + 3)
+    opts = [po for t in tiers for po in t]
+    if not any(po.name == "drf" for po in opts):
+        (tiers[-1] if tiers else tiers.append([]) or tiers[-1]).append(PluginOption.defaults("drf"))
+    for t in tiers:
+        for po in t:
+            if po.name == "drf":
+                po.hierarchy = True
+        names = [po.name for po in t]
+        if "drf" in names and "proportion" in names and rnd.random() < 0.5:  # the other tier order of the chain
+            i, k = names.index("drf"), names.index("proportion")
+            t[i], t[k] = t[k], t[i]
+    segs = ["d0", "d1", "t0", "t1", "t2"]
+    for q in tc.Queues:
+        depth = rnd.choice([0, 1, 1, 2, 2, 3, 4])
+        if depth == 0:
+            q.hierarchy, q.weights = rnd.choice([("", ""), ("root", "1")])
+            continue
+        q.hierarchy = "/".join(["root"] + [rnd.choice(segs) for _ in range(depth)])
+        q.weights = "/".join([str(rnd.choice([1, 100]))] + [rnd.choice(["1", "2", "5", "0.5", "abc", "0", "1.5", "0x2p0"])
+                                                              for _ in range(depth)])
+    return tc, tiers, actions, [q.hierarchy for q in tc.Queues], [q.weights for q in tc.Queues]
+
+
 def backfill_supported(tiers, conf_kw):
     """vc_backfill_run's documented limit: "pods" must not be a weighted hypernode-binpacking resource."""
     return not any(po.name == "network-topology-aware" and "pods" in str(po.arguments.get("hypernode.binpack.resources", ""))

@@ -198,6 +198,11 @@ class vc_hypernodes(C.Structure):
                 ("job_placed_off", C.POINTER(C.c_int32)), ("job_placed_node", C.POINTER(C.c_int32))]
 
 
+class vc_hdrf(C.Structure):
+    _fields_ = [("path_off", _i32p), ("path_name", _i32p), ("n_weights", _i32p), ("weight", _dp),
+                ("job_request", _dp)]
+
+
 class vc_running_tasks(C.Structure):
     _fields_ = [("n_tasks", C.c_int32), ("node", _i32p), ("job", _i32p), ("role", _i32p), ("priority", _i32p),
                 ("pod_index", _i64p), ("creation_ts", _i64p), ("uid_rank", C.POINTER(C.c_uint32)), ("resreq", _dp),
@@ -237,6 +242,7 @@ SYMBOLS = {
                                      C.POINTER(vc_jobs), C.POINTER(vc_queues), C.POINTER(vc_conf)]),
     "vc_snapshot_update_nodes": (C.c_int, [_vp, C.c_int32, _i32p, C.POINTER(vc_nodes)]),
     "vc_snapshot_set_topology": (C.c_int, [_vp, C.POINTER(vc_hypernodes)]),
+    "vc_snapshot_set_hdrf": (C.c_int, [_vp, C.POINTER(vc_hdrf)]),
     "vc_snapshot_set_backfill": (C.c_int, [_vp, C.c_int32, C.POINTER(vc_tasks)]),
     "vc_snapshot_set_running": (C.c_int, [_vp, C.POINTER(vc_running_tasks), C.POINTER(C.c_uint32)]),
     "vc_snapshot_set_nominated": (C.c_int, [_vp, C.POINTER(C.c_int32)]),

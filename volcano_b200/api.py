@@ -233,6 +233,8 @@ class Queue:
     state: str = "Open"
     creation_ts: int = 0
     reclaimable: bool = True  # Queue.Spec.Reclaimable (nil = true, api/queue_info.go:80-95)
+    hierarchy: str = ""  # volcano.sh/hierarchy annotation (QueueInfo.Hierarchy, api/queue_info.go:60)
+    weights: str = ""    # volcano.sh/hierarchy-weights annotation (QueueInfo.Weights, api/queue_info.go:61)
 
 
 @dataclass
@@ -318,6 +320,18 @@ def BuildPodGroupWithNetWorkTopologies(name, ns, hypernode_name, queue, min_memb
 
 def BuildQueue(name, weight, cap=None) -> Queue:
     return Queue(name=name, weight=weight, capability=dict(cap) if cap else None)
+
+
+KUBE_HIERARCHY_ANNOTATION_KEY = "volcano.sh/hierarchy"
+KUBE_HIERARCHY_WEIGHT_ANNOTATION_KEY = "volcano.sh/hierarchy-weights"
+
+
+def BuildQueueWithAnnos(name, weight, cap=None, annos=None) -> Queue:
+    """util.BuildQueueWithAnnos: a queue whose annotations carry the hdrf hierarchy and its weights."""
+    annos = annos or {}
+    return Queue(name=name, weight=weight, capability=dict(cap) if cap else None,
+                 hierarchy=annos.get(KUBE_HIERARCHY_ANNOTATION_KEY, ""),
+                 weights=annos.get(KUBE_HIERARCHY_WEIGHT_ANNOTATION_KEY, ""))
 
 
 def get_task_role(pod: Pod) -> str:

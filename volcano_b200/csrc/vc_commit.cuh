@@ -16,6 +16,7 @@
 // Bound: latency (mailbox round trip + fp64 dependency chain per step), not HBM — see DESIGN.md.
 #pragma once
 #include "vc_device.cuh"
+#include "vc_hdrf.hpp"
 
 struct HeapEnt {  // a re-pushed job with the key it had when pushed (keys are stable inside the PQ)
   double share;
@@ -23,6 +24,21 @@ struct HeapEnt {  // a re-pushed job with the key it had when pushed (keys are s
   int32_t prio;
   uint32_t rank;
   uint32_t bits;  // bit0 ready, bit1 preemptable
+};
+
+struct HdrfDev {  // device copy (global memory) of the tree (vc_hdrf.hpp), the order inputs and the per-CTA replica slab
+  int on;          // the queue PQ is simulated as a Go heap under the hdrf comparator chain
+  int M, n_init, R, J, Q;
+  vch::HdrfOrder ord;
+  const int32_t *parent, *child_off, *child, *j_node, *q_path_off, *q_path, *q_init;
+  const double *weight, *j_req;
+  const int32_t *q_prio;
+  const uint32_t *q_rank;
+  double total[VC_MAX_DIMS];
+  uint32_t total_has;
+  double tot0[VC_MAX_DIMS];  // drf.totalAllocated at open
+  unsigned char *rep;
+  size_t rep_stride;
 };
 
 struct K2Params {
@@ -120,7 +136,84 @@ struct K2Params {
   int32_t *job_alloc_out;     // [J] subJob.AllocatedHyperNode after the run
   int topo_nval;              // distinct values networkTopologyAwareScore can take, ascending
   double topo_val[VC_MAX_TIERS + 2];
+  // ---- hierarchical drf (vc_snapshot_set_hdrf): the queue PQ becomes a simulated Go heap ----
+  int hd_on;
+  const HdrfDev *hd;  // device memory
 };
+
+// Per-CTA replica of the hdrf tree and of the queue heap, and where the kernel's own replica keeps the jobs' drf state
+// and the queues' proportion shares (the two kernels lay them out differently). The functions below run on one thread and
+// are not inlined: the control program only pays for a call where hdrf is configured.
+struct HdrfAcc {
+  const double *ja; long long ja_sj, ja_sd;  // job allocation
+  const double *js; long long js_sj;         // job share
+  const double *qs; long long qs_q;          // proportion share of queue q
+};
+struct HdrfRep { double *n_alloc, *n_share, *tot; int32_t *n_sat, *j_sat, *heap, *dem; HdrfAcc *acc; };
+__device__ __forceinline__ HdrfRep hd_rep(const HdrfDev *h, int lcta) {
+  unsigned char *b = h->rep + (size_t)lcta * h->rep_stride;
+  HdrfRep r;
+  r.acc = reinterpret_cast<HdrfAcc *>(b); b += (sizeof(HdrfAcc) + 15) & ~(size_t)15;
+  r.n_alloc = reinterpret_cast<double *>(b); b += (size_t)h->M * h->R * 8;
+  r.n_share = reinterpret_cast<double *>(b); b += (size_t)h->M * 8;
+  r.tot = reinterpret_cast<double *>(b); b += (size_t)VC_MAX_DIMS * 8;
+  r.n_sat = reinterpret_cast<int32_t *>(b); b += (size_t)h->M * 4;
+  r.j_sat = reinterpret_cast<int32_t *>(b); b += (size_t)h->J * 4;
+  r.heap = reinterpret_cast<int32_t *>(b); b += (size_t)h->Q * 4;
+  r.dem = reinterpret_cast<int32_t *>(b);
+  return r;
+}
+__device__ __forceinline__ vch::HdrfView hd_view(const HdrfDev *h, const HdrfRep &r) {
+  const HdrfAcc &a = *r.acc;
+  vch::HdrfView v;
+  v.R = h->R; v.M = h->M; v.J = h->J;
+  v.parent = h->parent; v.child_off = h->child_off; v.child = h->child; v.j_node = h->j_node; v.j_req = h->j_req;
+  v.j_alloc = a.ja; v.ja_sj = a.ja_sj; v.ja_sd = a.ja_sd; v.j_share = a.js; v.js_sj = a.js_sj;
+  v.total = h->total; v.total_has = h->total_has;
+  v.n_alloc = r.n_alloc; v.n_share = r.n_share; v.n_sat = r.n_sat; v.j_sat = r.j_sat; v.tot = r.tot; v.dem = r.dem;
+  return v;
+}
+struct HdLess {  // ssn.QueueOrderFn on the replica: the hdrf / proportion chain, then the (CreationTimestamp, UID) rank
+  const HdrfDev *h;
+  HdrfRep r;
+  __host__ __device__ int prio(int q) const { return h->q_prio[q]; }
+  __host__ __device__ double share(int q) const { return r.acc->qs[q * r.acc->qs_q]; }
+  __host__ __device__ uint32_t rank(int q) const { return h->q_rank[q]; }
+  __host__ __device__ bool operator()(int l, int rr) const {
+    return vch::hdrf_queue_less(h->ord, h->q_path_off, h->q_path, h->weight, r.n_share, r.n_sat, *this, l, rr);
+  }
+};
+// the tree at session open and queues.Push of every queue of buildAllocateContext (allocate.go:185-188), in the order the
+// queues first appear over the jobs; returns the heap size
+__device__ __noinline__ int hd_open(const HdrfDev *h, int lcta, const double *ja, long long ja_sj, long long ja_sd,
+                                    const double *js, long long js_sj, const double *qs, long long qs_q) {
+  const HdrfRep r = hd_rep(h, lcta);
+  r.acc->ja = ja; r.acc->ja_sj = ja_sj; r.acc->ja_sd = ja_sd; r.acc->js = js; r.acc->js_sj = js_sj; r.acc->qs = qs; r.acc->qs_q = qs_q;
+  for (int d = 0; d < VC_MAX_DIMS; ++d) r.tot[d] = h->tot0[d];
+  r.dem[0] = -1;
+  vch::hdrf_refresh(hd_view(h, r), -1);
+  const HdLess less{h, r};
+  int n = 0;
+  for (int k = 0; k < h->n_init; ++k) vch::qheap_push(r.heap, n, h->q_init[k], less);
+  return n;
+}
+// queues.Pop() on the heap as it is (the tree is current: nothing changed since the last push)
+__device__ __noinline__ int hd_pop(const HdrfDev *h, int lcta, int n) {
+  const HdrfRep r = hd_rep(h, lcta);
+  const HdLess less{h, r};
+  return vch::qheap_pop(r.heap, n, less);
+}
+// drf.totalAllocated follows a visit's events (integer-valued: exact in any order)
+__device__ __noinline__ void hd_tot_add(const HdrfDev *h, int lcta, int d, double delta) { hd_rep(h, lcta).tot[d] += delta; }
+// queues.Push(queue) after a visit of `job` (allocate.go:346): bring the tree up to the events of the visit (the replica's
+// job records and totalAllocated are already current), then sift up; returns the heap size
+__device__ __noinline__ int hd_push(const HdrfDev *h, int lcta, int n, int job, int q) {
+  const HdrfRep r = hd_rep(h, lcta);
+  vch::hdrf_refresh(hd_view(h, r), job);
+  const HdLess less{h, r};
+  vch::qheap_push(r.heap, n, q, less);
+  return n;
+}
 
 // ---------------------------------------------------------------------------------------
 // shared-memory resident node slice of one CTA
@@ -720,6 +813,9 @@ __global__ void __launch_bounds__(256, 1) k_commit(K2Params p) {
     S.prof_last = clock64();
   }
   __syncthreads();
+  // hdrf: the queue PQ is a simulated Go heap (thread 0), its comparator reads the tree replica
+  int hd_n = 0;
+  if (p.hd_on && tid == 0) hd_n = hd_open(p.hd, cta, j_alloc, 1, J, j_share, 1, q_share, 1);
 
   const bool out_cta = (cta == 0);  // CTA 0 writes the result lists
   const bool qorder_prop = [&] {
@@ -739,7 +835,12 @@ __global__ void __launch_bounds__(256, 1) k_commit(K2Params p) {
   for (;;) {
     // ---- queues.Pop(): arg-min over the active queues by ssn.QueueOrderFn (session_plugins.go:709-731;
     //      proportion: priority desc, then share asc — proportion.go:266-284; then (ts, uid) rank)
-    if (warp == 0) {
+    if (p.hd_on) {
+      if (tid == 0) {
+        S.pick = hd_n > 0 ? hd_pop(p.hd, cta, hd_n) : -1;
+        hd_n = hd_n > 0 ? hd_n - 1 : 0;
+      }
+    } else if (warp == 0) {
       int bq = -1, bprio = 0;
       double bshare = 0.0;
       uint32_t brank = 0;
@@ -1376,6 +1477,8 @@ __global__ void __launch_bounds__(256, 1) k_commit(K2Params p) {
         j_nplaced[j] = S.nplaced;
         if (ready && S.job_soft) j_alloc_hn[j] = S.topo_A;  // subJob.AllocatedHyperNode = allocatedHyperNode, :681-686
       }
+      if (p.hd_on)
+        for (int d = 0; d < R; ++d) hd_tot_add(p.hd, cta, d, S.jalloc[d] - j_alloc[(size_t)d * J + j]);
       for (int d = 0; d < R; ++d) j_alloc[(size_t)d * J + j] = S.jalloc[d];
       for (int r = 0; r < S.nroles; ++r) {
         int gr = S.role_base + r;
@@ -1421,6 +1524,7 @@ __global__ void __launch_bounds__(256, 1) k_commit(K2Params p) {
         h[i] = e;
       }
       q_active[q] = 1;  // queues.Push(queue), allocate.go:346
+      if (p.hd_on) hd_n = hd_push(p.hd, cta, hd_n, j, q);
     }
     __syncthreads();
     PROF_MARK(0);

@@ -1029,6 +1029,16 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
     // warps read. Per-dimension vectors (drf / proportion accumulators) live one dimension per lane.
     // ===================================================================================
     const bool out_cta = (cta == 0);
+    // hdrf: the queue PQ is a simulated Go heap run by lane 0 on the tree replica; hd_n (its size) is kept in every lane
+    int hd_n = 0;
+    if (p.hd_on) {
+      if (lane == 0)
+        hd_n = hd_open(p.hd, lcta, reinterpret_cast<const double *>(reinterpret_cast<const char *>(jdyn) + offsetof(JobDyn, alloc)),
+                       sizeof(JobDyn) / 8, 1, reinterpret_cast<const double *>(reinterpret_cast<const char *>(jdyn) + offsetof(JobDyn, share)),
+                       sizeof(JobDyn) / 8, reinterpret_cast<const double *>(reinterpret_cast<const char *>(qdyn) + offsetof(QueueDyn, share)),
+                       sizeof(QueueDyn) / 8);
+      hd_n = __shfl_sync(0xffffffffu, hd_n, 0);
+    }
     // ---- register copies of the control state ----
     int cur_group = -1, cache_group = -1, since_sync = 0;
     unsigned ag = 0, pc = 0;
@@ -1074,6 +1084,12 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
       int bq = -1, bprio = 0;
       double bshare = 0.0;
       uint32_t brank = 0;
+      if (p.hd_on) {  // hdrf: heap.Pop under the comparator chain on the tree as it is
+        int qq = -1;
+        if (lane == 0 && hd_n > 0) qq = hd_pop(p.hd, lcta, hd_n);
+        bq = __shfl_sync(0xffffffffu, qq, 0);
+        hd_n = hd_n > 0 ? hd_n - 1 : 0;
+      } else {
       for (int q = lane; q < Q; q += 32) {
         if (!(q_mirror ? F.q_active[q] : qdyn[q].active)) continue;
         int pr = f_qorder_prop ? __ldg(&fp.qstat[q].prio) : 0;
@@ -1089,6 +1105,7 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
         uint32_t ork = __shfl_xor_sync(0xffffffffu, brank, o);
         bool lt = oq >= 0 && (bq < 0 || opr > bprio || (opr == bprio && (osh < bshare || (osh == bshare && ork < brank))));
         if (lt) { bq = oq; bprio = opr; bshare = osh; brank = ork; }
+      }
       }
       const int q = bq;
       if (q < 0) break;
@@ -1822,8 +1839,9 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
             // The visit ends with this placement, the statement commits and the job is pushed back with the key it was
             // popped with (Ready bit set, no drf share in ssn.JobOrderFn): it is the head of its queue again. The
             // queue is popped again when ssn.QueueOrderFn does not depend on the share or no other queue is active.
-            bool again = !f_qorder_prop;
-            if (!again) {
+            // hdrf: the shares move with every placement, so only an otherwise empty heap pops the queue again
+            bool again = p.hd_on ? hd_n == 0 : !f_qorder_prop;
+            if (!again && !p.hd_on) {
               const int na = __popc(__ballot_sync(0xffffffffu, lane < Q && F.q_active[lane] != 0)) +
                              __popc(__ballot_sync(0xffffffffu, lane + 32 < Q && F.q_active[lane + 32] != 0));
               again = na <= 1;  // (the queue of this visit is marked inactive while it is being served or is the one)
@@ -2032,6 +2050,9 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
       }
       // ---- write the job / queue / role records back into the replica ----
       __syncwarp();
+      // hdrf: drf.totalAllocated follows the visit's events (integer-valued: exact in any order)
+      if (p.hd_on && lane < R) hd_tot_add(p.hd, lcta, lane, jalloc_l - jdyn[j].alloc[lane]);
+      __syncwarp();
       if (lane == 0) {
         JobDyn *jd = &jdyn[j];
         jd->ready = ready; jd->waiting = waiting; jd->cursor = cursor - task_off; jd->share = jshare;
@@ -2047,6 +2068,11 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
         rdyn[role_base + r] = rd;
       }
       __syncwarp();
+      if (p.hd_on) {  // queues.Push(queue) on the heap, after the tree caught up with the visit
+        int nn = 0;
+        if (lane == 0) nn = hd_push(p.hd, lcta, hd_n, j, q);
+        hd_n = __shfl_sync(0xffffffffu, nn, 0);
+      }
       FPROF_MARK(0);
     }
     if (pub_pending && pub_owner == cta) asm volatile("bar.sync 1, 64;" ::: "memory");  // pair the evaluator's last arrive

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../include/vcalloc.h"
+#include "vc_hdrf.hpp"
 
 namespace vch {
 
@@ -348,13 +349,19 @@ inline void rank_by(const int64_t *ts, const uint32_t *uid, size_t n, std::vecto
   rank.resize(n);
   for (size_t r = 0; r < n; ++r) rank[idx[r]] = (uint32_t)r;
 }
+// hdrf (drf's enableHierarchy) for the pick order: the tree built at upload and TotalRequest [R][J]
+struct HdrfPick {
+  const HdrfTree *tree;
+  const double *job_request;
+};
 // `ops`: the operations of the preceding allocate action (kept visits only, in order); task_*: allocate's task arrays.
 // `alloc_ran`: allocate ran before in this session. Without the enqueue action its buildAllocateContext rewrites the phase of
 // every Pending PodGroup to Inqueue (allocate.go:154-164), so job.IsPending() (backfill.go:124) is false afterwards.
 inline BackfillPick backfill_pick(const vc_conf &conf, bool alloc_ran, size_t R, size_t T, size_t J, size_t Q, size_t B, bool has_drf,
                                   bool has_proportion, const double *total, uint32_t total_has, const BackfillTasks &bf,
                                   const BackfillKeep &bk, const vc_decision *ops_p, size_t n_ops, const int32_t *task_job,
-                                  const double *task_req, const uint32_t *task_has, std::vector<QAttr> qattr) {
+                                  const double *task_req, const uint32_t *task_has, std::vector<QAttr> qattr,
+                                  const HdrfPick *hd = nullptr) {
   struct OpsView { const vc_decision *b, *e; const vc_decision *begin() const { return b; } const vc_decision *end() const { return e; } };
   const OpsView ops{ops_p, ops_p + n_ops};
   // ---- 1. the session state the allocate action left: ready counts, role occupancy, drf / proportion shares ----
@@ -413,7 +420,21 @@ inline BackfillPick backfill_pick(const vc_conf &conf, bool alloc_ran, size_t R,
     return bk.j_rank[l] < bk.j_rank[rr];
   };
   const bool qorder_prop = plugin_enabled(conf, VC_PLUGIN_PROPORTION, VC_EN_QUEUE_ORDER);
+  // hdrf: the tree on the state allocate left (every order function is evaluated before backfill places anything)
+  const HdrfOrder hd_ord = hdrf_order(conf);
+  const bool hd_on = hd && has_drf && hd_ord.hdrf_on;
+  HdrfState hst;
+  if (hd_on) hdrf_eval(*hd->tree, (int)R, (int)J, total, total_has, j_alloc.data(), j_share.data(), hd->job_request, hst);
+  struct QV {
+    const BackfillKeep &bk; const std::vector<double> &q_share;
+    int prio(int q) const { return bk.q_prio[q]; }
+    double share(int q) const { return q_share[q]; }
+    uint32_t rank(int q) const { return bk.q_rank[q]; }
+  } qv{bk, q_share};
   auto queue_less = [&](int l, int rr) {  // ssn.QueueOrderFn :709-731; proportion.go:266-284
+    if (hd_on)
+      return hdrf_queue_less(hd_ord, hd->tree->q_path_off.data(), hd->tree->q_path.data(), hd->tree->weight.data(),
+                             hst.n_share.data(), hst.n_sat.data(), qv, l, rr);
     if (qorder_prop) {
       if (bk.q_prio[l] != bk.q_prio[rr]) return bk.q_prio[l] > bk.q_prio[rr];
       if (q_share[l] != q_share[rr]) return q_share[l] < q_share[rr];

@@ -253,6 +253,16 @@ struct vc_snapshot {
   int32_t *d_nominated = nullptr;
   size_t d_nominated_cap = 0;
   bool fut_rows = false;  // Releasing / Pipelined resources present at open
+  // ---- hierarchical drf (vc_snapshot_set_hdrf) ----
+  bool hd_set = false;
+  std::vector<int32_t> hd_path_off, hd_path_name, hd_nw;
+  std::vector<double> hd_weight, hd_jreq;
+  vch::HdrfTree hd_tree;
+  HdrfDev hdp{};            // device view of the tree, filled at upload (hdp.on: queue order by hdrf)
+  void *d_hd = nullptr;     // device copy of the tree tables
+  HdrfDev *d_hdp = nullptr; // device copy of hdp (with the replica slab of the last run)
+  unsigned char *rep_hd = nullptr;  // per-CTA tree replicas + queue heaps
+  size_t rep_hd_bytes = 0;
   bool all_pure = true;  // every job's named roles map to one (class, request) group each: the role-keyed error cache is a no-op
   bool rows_integral = false;  // every quantity a placement adds to / subtracts from a node row is integer-valued
   void *d_bf = nullptr;   // device slab of the backfill inputs / outputs
@@ -491,7 +501,7 @@ void vc_snapshot_destroy(vc_snapshot *s) {
     if (r != s->rank && s->peer_comm[r]) cudaIpcCloseMemHandle(s->peer_comm[r]);
   if (s->comm) cudaFree(s->comm);
   void *dptrs[] = {s->in.dev, s->cstat, s->w_idle, s->w_used, s->w_pip, s->w_kreq, s->w_knz, s->w_pod_count,
-                   s->rep_i32, s->rep_f64, s->rep_heap, s->rep_hn_used, s->rep_placed, s->d_job_alloc, s->hn_score, s->mbox, s->ring, s->d_score_log, s->d_prof, s->d_wait, s->d_dbg, s->d_nominated, s->d_decisions, s->d_visits, s->d_fit, s->d_counters, s->d_bf, s->w_rel, s->d_ev};
+                   s->rep_i32, s->rep_f64, s->rep_heap, s->rep_hn_used, s->rep_placed, s->d_job_alloc, s->hn_score, s->mbox, s->ring, s->d_score_log, s->d_prof, s->d_wait, s->d_dbg, s->d_nominated, s->d_decisions, s->d_visits, s->d_fit, s->d_counters, s->d_bf, s->w_rel, s->d_ev, s->d_hd, s->rep_hd, s->d_hdp};
   for (void *p : dptrs) if (p) cudaFree(p);
   void *hptrs[] = {s->in.pin, s->h_decisions, s->h_visits, s->h_fit, s->h_counters, s->h_ev, s->delta_pin};
   if (s->delta_dev) cudaFree(s->delta_dev);
@@ -1001,6 +1011,56 @@ int vc_snapshot_upload(vc_snapshot *s, const vc_nodes *nd, const vc_tasks *tk, c
   }
   // network-topology-aware: hyperNodeResourceCache at open (network_topology_aware.go:106-125) and, for the
   // commit kernel, the hypernodes each CTA's node slice belongs to
+  // hierarchical drf: the tree after session open inserted every job (drf.go:186-220), its device tables
+  s->hdp = HdrfDev{};
+  if (s->hd_set) {
+    if (!s->dc.has_drf) return fail(VC_EINVAL, "hdrf table without the drf plugin");
+    const std::string why = vch::hdrf_build((int)J, (int)Q, jb->queue, vc_hdrf{s->hd_path_off.data(), s->hd_path_name.data(),
+                                            s->hd_nw.data(), s->hd_weight.data(), s->hd_jreq.data()}, s->hd_tree);
+    if (!why.empty()) return fail(VC_EINVAL, "hdrf: %s", why.c_str());
+    // the replicas keep drf.totalAllocated by adding each visit's change and recompute the tree lazily: exact when every
+    // quantity is an integer (SURVEY Appendix A-2)
+    double mx = 0;
+    if (!vch::max_abs_integral(tk->resreq, R * T, mx) || !vch::max_abs_integral(jb->allocated, R * J, mx) ||
+        !vch::max_abs_integral(s->hd_jreq.data(), R * J, mx))
+      return fail(VC_EINVAL, "hdrf: task requests, job allocations and job requests must be integer-valued");
+    const vch::HdrfTree &t = s->hd_tree;
+    std::vector<int32_t> q_init;  // buildAllocateContext pushes a queue when its first job is pushed (job index order)
+    for (size_t q = 0; q < Q; ++q) if (!qlists[q].empty()) q_init.push_back((int32_t)q);
+    auto first_job = [&](int q) { return *std::min_element(qlists[q].begin(), qlists[q].end()); };
+    std::sort(q_init.begin(), q_init.end(), [&](int a, int b) { return first_job(a) < first_job(b); });
+    // one device blob: ints then doubles
+    std::vector<int32_t> iv;
+    auto put_i = [&](const std::vector<int32_t> &v) { size_t o = iv.size(); iv.insert(iv.end(), v.begin(), v.end()); return o; };
+    const size_t o_par = put_i(t.parent), o_coff = put_i(t.child_off), o_ch = put_i(t.child), o_jn = put_i(t.j_node),
+                 o_qpo = put_i(t.q_path_off), o_qp = put_i(t.q_path), o_qi = put_i(q_init);
+    const size_t ibytes = (iv.size() * 4 + 15) & ~(size_t)15;
+    const size_t bytes = ibytes + (t.weight.size() + R * J) * 8;
+    if (s->d_hd) cudaFree(s->d_hd);
+    s->d_hd = nullptr;
+    CUDA_TRY(cudaMalloc(&s->d_hd, std::max<size_t>(bytes, 16)));
+    unsigned char *db = static_cast<unsigned char *>(s->d_hd);
+    CUDA_TRY(cudaMemcpy(db, iv.data(), iv.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(db + ibytes, t.weight.data(), t.weight.size() * 8, cudaMemcpyHostToDevice));
+    if (R * J) CUDA_TRY(cudaMemcpy(db + ibytes + t.weight.size() * 8, s->hd_jreq.data(), R * J * 8, cudaMemcpyHostToDevice));
+    const int32_t *di = reinterpret_cast<const int32_t *>(db);
+    HdrfDev &h = s->hdp;
+    h.ord = vch::hdrf_order(*conf);
+    h.on = h.ord.hdrf_on;  // hdrf's queueOrderFn is dispatched only with drf's EnabledQueueOrder
+    h.M = t.M; h.n_init = (int)q_init.size();
+    h.parent = di + o_par; h.child_off = di + o_coff; h.child = di + o_ch; h.j_node = di + o_jn;
+    h.q_path_off = di + o_qpo; h.q_path = di + o_qp; h.q_init = di + o_qi;
+    h.weight = reinterpret_cast<const double *>(db + ibytes);
+    h.j_req = h.weight + t.weight.size();
+    for (size_t d = 0; d < VC_MAX_DIMS; ++d) {
+      double acc = 0;
+      if (d < R) for (size_t j = 0; j < J; ++j) acc += jb->allocated[d * J + j];
+      h.tot0[d] = acc;
+      h.total[d] = s->total[d];
+    }
+    h.total_has = s->total_has;
+    h.R = (int)R; h.J = (int)J; h.Q = (int)Q;
+  }
   choose_geometry(s);
   if (s->n_cta_total > 2048) return fail(VC_EUNSUPPORTED, "too many CTAs (%d)", s->n_cta_total);
   if (s->world > 1 && !s->fast)
@@ -1518,6 +1578,25 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
     CUDA_TRY(cudaMemsetAsync(d_wait, 0, 1024 * 8, s->stream));
   }
   p.cta_wait = d_wait;
+  p.hd_on = s->hdp.on;
+  p.hd = nullptr;
+  if (p.hd_on) {  // per-CTA tree replica + queue heap (hd_rep in vc_commit.cuh)
+    HdrfDev hd = s->hdp;
+    const size_t per = (((sizeof(HdrfAcc) + 15) & ~(size_t)15) + ((size_t)hd.M * R + hd.M + VC_MAX_DIMS) * 8 +
+                        ((size_t)hd.M + J + Q + 1) * 4 + 15) & ~(size_t)15;
+    if (s->rep_hd_bytes < per * G) {
+      if (s->rep_hd) cudaFree(s->rep_hd);
+      s->rep_hd = nullptr;
+      CUDA_TRY(cudaMalloc(&s->rep_hd, per * G));
+      s->rep_hd_bytes = per * G;
+    }
+    hd.rep = s->rep_hd; hd.rep_stride = per;
+    hd.q_prio = p.q_prio; hd.q_rank = p.q_rank;
+    if (!s->d_hdp) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&s->d_hdp), sizeof(HdrfDev)));
+    CUDA_TRY(cudaMemcpyAsync(s->d_hdp, &hd, sizeof hd, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));  // `hd` is a stack copy
+    p.hd = s->d_hdp;
+  }
   // (the instrumented instance exists for the plain and the FUT shape)
   const void *kfn = s->fast && s->dc.to_find > 0 ? (s->fut_rows ? (const void *)k_commit_fast<false, true, false, true>
                                                                  : g_tun.prof ? (const void *)k_commit_fast<true, false, false, true> : (const void *)k_commit_fast<false, false, false, true>)
@@ -1811,6 +1890,8 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   if (!s->uploaded) return fail(VC_EINVAL, "vc_snapshot_upload must precede the action");
   if (s->any_nominated)
     return fail(VC_EUNSUPPORTED, "preempt / reclaim: a pending task carries a NominatedNodeName (taskEligibleToPreempt's rules are not modelled)");
+  if (s->hd_set)
+    return fail(VC_EUNSUPPORTED, "preempt / reclaim with drf's enableHierarchy: the hdrf tree on evict events and hdrf's reclaimFn (drf.go:280-367) are not built");
   const double t0 = now_ms();
   int rc = ensure_evict_session(s);
   if (rc) return rc;
@@ -2123,6 +2204,27 @@ int vc_reclaim_run(vc_snapshot *s, vc_result **out) { return run_evict_action(s,
 // ---------------------------------------------------------------------------------------
 // backfill (actions/backfill/backfill.go)
 // ---------------------------------------------------------------------------------------
+int vc_snapshot_set_hdrf(vc_snapshot *s, const vc_hdrf *h) {
+  if (!s) return fail(VC_EINVAL, "null snapshot");
+  s->uploaded = false;  // the tree is built at upload: the session must be uploaded again
+  s->hd_set = false;
+  if (!h) return VC_OK;
+  const size_t Q = s->dims.n_queues, J = s->dims.n_jobs, R = s->dims.n_dims;
+  if (!h->path_off || !h->n_weights || (J > 0 && !h->job_request)) return fail(VC_EINVAL, "hdrf table: missing arrays");
+  if (h->path_off[0] != 0) return fail(VC_EINVAL, "hdrf table: path_off[0] must be 0");
+  for (size_t q = 0; q < Q; ++q)
+    if (h->path_off[q + 1] < h->path_off[q]) return fail(VC_EINVAL, "hdrf table: path_off not monotone at queue %zu", q);
+  const size_t P = (size_t)h->path_off[Q];
+  if (P > 0 && (!h->path_name || !h->weight)) return fail(VC_EINVAL, "hdrf table: missing path arrays");
+  s->hd_path_off.assign(h->path_off, h->path_off + Q + 1);
+  s->hd_path_name.assign(h->path_name, h->path_name + P);
+  s->hd_weight.assign(h->weight, h->weight + P);
+  s->hd_nw.assign(h->n_weights, h->n_weights + Q);
+  s->hd_jreq.assign(h->job_request, h->job_request + R * J);
+  s->hd_set = true;
+  return VC_OK;
+}
+
 int vc_snapshot_set_nominated(vc_snapshot *s, const int32_t *nominated_node) {
   if (!s) return fail(VC_EINVAL, "null snapshot");
   s->uploaded = false;  // validated against the node table and shipped by the next upload
@@ -2180,9 +2282,11 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
   const vc_conf &conf = s->conf;
 
   // ---- 1 + 2. session state after allocate and pickUpPendingTasks (backfill.go:118-199): vc_host.hpp ----
+  const vch::HdrfPick hd_pick{&s->hd_tree, s->hd_jreq.data()};  // hdrf: the tree as of the last upload
   vch::BackfillPick pick = vch::backfill_pick(conf, s->alloc_ran, R, T, J, Q, B, s->dc.has_drf != 0, s->dc.has_proportion != 0, s->total,
                                               s->total_has, bf, bk, s->last_dec.data(), s->last_dec.size(), s->ek.t_job.data(),
-                                              s->ek.t_req.data(), s->ek.t_has.data(), s->qattr);
+                                              s->ek.t_req.data(), s->ek.t_has.data(), s->qattr,
+                                              s->hd_set ? &hd_pick : nullptr);
   const std::vector<int32_t> &order = pick.order, &j_ready = pick.j_ready, &r_occ = pick.r_occ;
   const std::vector<int> &visit_job = pick.visit_job, &visit_begin = pick.visit_begin;
   auto is_ready = [&](int j) { return j_ready[j] + bk.j_pbe[j] >= bk.j_min[j]; };  // job_info.go:1169

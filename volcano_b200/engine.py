@@ -89,6 +89,8 @@ class Engine:
         topo = s.topology()
         if topo is not None:
             _check(self.L.vc_snapshot_set_topology(self.h, C.byref(topo)))
+        hd = s.hdrf()  # drf's enableHierarchy: restated on every upload, None clears it
+        _check(self.L.vc_snapshot_set_hdrf(self.h, C.byref(hd) if hd is not None else None))
         bt = s.backfill_tasks()  # the list stays in effect until replaced: always (re)state it, an empty one clears it
         _check(self.L.vc_snapshot_set_backfill(self.h, s.B, C.byref(bt) if bt is not None else None))
         rt = s.running_tasks()  # node.Tasks (victim candidates of preempt / reclaim) + per-task flags; restated on every upload

@@ -9,10 +9,9 @@ i.e. exactly the marshalling the cgo shim performs in Go (INTEGRATION.md).
 from __future__ import annotations
 
 import ctypes as C
+import re
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
-
-import re
 
 import numpy as np
 
@@ -30,21 +29,23 @@ class PluginOption:
     name: str
     enabled: int = 0  # OR of abi.VC_EN_*; 0 mirrors the reference's nil pointers in unit tests
     arguments: Dict[str, object] = field(default_factory=dict)
+    hierarchy: bool = False  # EnabledHierarchy (drf: hierarchical drf, plugins/drf/drf.go:147-158)
 
     @staticmethod
     def make(name: str, arguments: Optional[Dict[str, object]] = None, **enables: bool) -> "PluginOption":
         """PluginOption{Name: ..., EnabledJobOrder: &trueValue, ...}."""
         flags = 0
+        hierarchy = False
         for k, v in enables.items():
-            if k.lower() in ("enabledhierarchy", "enablehierarchy") and v:
-                # hierarchical drf (plugins/drf/drf.go:147-156, hdrf) orders queues by a tree the path does not model
-                raise NotImplementedError("drf with enableHierarchy (hdrf) is outside the accelerated path")
+            if k.lower() in ("enabledhierarchy", "enablehierarchy"):
+                hierarchy = bool(v)
+                continue
             if k not in abi.ENABLE_FLAGS:
                 # extension points that do not touch the allocate path (EnabledPreemptable, ...)
                 continue
             if v:
                 flags |= abi.ENABLE_FLAGS[k]
-        return PluginOption(name=name, enabled=flags, arguments=dict(arguments or {}))
+        return PluginOption(name=name, enabled=flags, arguments=dict(arguments or {}), hierarchy=hierarchy)
 
     @staticmethod
     def defaults(name: str, arguments: Optional[Dict[str, object]] = None) -> "PluginOption":
@@ -301,6 +302,34 @@ class Snapshot:
         self.job_names: List[str] = []
         self.queue_names: List[str] = []
 
+    def hdrf(self) -> Optional[abi.vc_hdrf]:
+        """drf's enableHierarchy table (None: the option is off)."""
+        if getattr(self, "hd_path_off", None) is None:
+            return None
+        return abi.vc_hdrf(_ptr(self.hd_path_off, _I32), _ptr(self.hd_path_name, _I32), _ptr(self.hd_n_weights, _I32),
+                           _ptr(self.hd_weight, _F64), _ptr(self.hd_job_request, _F64))
+
+    def set_hdrf(self, hierarchy: Sequence[str], weights: Sequence[str], job_request: np.ndarray) -> None:
+        """Encode QueueInfo.Hierarchy / Weights of every queue (split on "/", the root segment dropped; names
+        interned, weights through strconv.ParseFloat) and JobInfo.TotalRequest ([R][J])."""
+        names: Dict[str, int] = {}
+        off, pn, nw, wt = [0], [], [], []
+        for h, w in zip(hierarchy, weights):
+            segs, ws = h.split("/")[1:], w.split("/")[1:]
+            for i, seg in enumerate(segs):
+                pn.append(names.setdefault(seg, len(names)))
+                wt.append(go_parse_float(ws[i]) if i < len(ws) else 0.0)
+            nw.append(len(ws))
+            off.append(len(pn))
+        self.hd_path_off = np.array(off, np.int32)
+        self.hd_path_name = np.array(pn, np.int32)
+        self.hd_n_weights = np.array(nw, np.int32)
+        self.hd_weight = np.array(wt, np.float64)
+        self.hd_job_request = np.ascontiguousarray(job_request, np.float64).reshape(self.R, self.J)
+
+    def clear_hdrf(self) -> None:
+        self.hd_path_off = None
+
     def topology(self) -> Optional[abi.vc_hypernodes]:
         if self.hn_member is None:
             return None
@@ -432,6 +461,40 @@ class Snapshot:
 _K8S_DEFAULT_MILLI_CPU = 100           # schedutil.DefaultMilliCPURequest
 _K8S_DEFAULT_MEMORY = 200 * 1024 * 1024  # schedutil.DefaultMemoryRequest
 KDIM_NAMES = ("cpu", "memory", "nvidia.com/gpu")  # nodeorder.go:238-244
+
+
+_GO_DEC = re.compile(r"[+-]?(?:\d+\.?\d*|\.\d+)(?:[eE][+-]?\d+)?")
+_GO_HEX = re.compile(r"([+-]?)0[xX]((?:[0-9a-fA-F_]+\.?[0-9a-fA-F_]*|\.[0-9a-fA-F_]+))[pP]([+-]?[0-9_]+)")
+_GO_SPECIAL = re.compile(r"[+-]?(?:inf|infinity)|nan", re.IGNORECASE)
+
+
+def _underscores_ok(s: str) -> bool:
+    """strconv's underscoreOK for a base-prefixed number: every '_' sits between two digits or right after the prefix."""
+    for i, ch in enumerate(s):
+        if ch != "_":
+            continue
+        prev, nxt = s[i - 1] if i else "", s[i + 1] if i + 1 < len(s) else ""
+        if not (prev.isalnum() and nxt.isalnum()) or prev in "pP" or nxt in "pP":
+            return False
+    return True
+
+
+def go_parse_float(text: str) -> float:
+    """The value strconv.ParseFloat(text, 64) returns, error or not: 0 for a syntax error, +-Inf out of range. Decimal and
+    hexadecimal (0x mantissa, p exponent) forms, inf / infinity with a sign, nan without one; underscores only in the
+    base-prefixed form."""
+    if _GO_SPECIAL.fullmatch(text) or _GO_DEC.fullmatch(text):
+        return float(text)  # Python's float() rounds like Go's; an overflow gives +-inf as ParseFloat does
+    m = _GO_HEX.fullmatch(text)
+    if m and _underscores_ok(text):
+        sign, mant, exp = m.group(1), m.group(2).replace("_", ""), m.group(3).replace("_", "")
+        if not any(c not in "." for c in mant):
+            return 0.0
+        try:
+            return float.fromhex(f"{sign}0x{mant}p{exp}")
+        except OverflowError:
+            return float("-inf") if sign == "-" else float("inf")
+    return 0.0
 
 
 def _resource_vector(rl: Optional[Dict[str, str]], dim_names: Sequence[str]):
@@ -953,4 +1016,11 @@ def encode_cluster(nodes: Sequence[Node], pods: Sequence[Pod], podgroups: Sequen
     s.actions = tuple(conf.actions)
     if hypernodes is not None:
         encode_hypernodes(s, hypernodes, podgroups, job_pods)
+    if any(p.hierarchy for tier in conf.tiers for p in tier if p.name == "drf"):
+        # JobInfo.TotalRequest: Resreq of every task of the job, any status (api/job_info.go:640-648)
+        treq = np.zeros((R, J))
+        for j in range(J):
+            for p in job_pods[j]:
+                treq[:, j] += pod_req(p)[0]
+        s.set_hdrf([q.hierarchy for q in queues], [q.weights for q in queues], treq)
     return s

@@ -42,6 +42,7 @@ class SynthConfig:
     n_besteffort: int = 0             # extra BestEffort pending pods spread over the jobs (the backfill action's tasks)
     hetero: int = 0                   # > 0: every task draws its own request from `hetero` distinct cpu / memory sizes
                                       # (heterogeneous pods: the (class, request) groups of the dense pass approach T)
+    hdrf: Optional[tuple] = None      # (departments, teams): drf's enableHierarchy over a root -> department -> team tree
 
 
 CONFIGS = {
@@ -65,6 +66,9 @@ CONFIGS = {
                             utilisation=0.9, min_util=0.5, releasing_frac=0.4),
     # configs[2]: + DRF + proportion over 16 queues
     "cfg3": SynthConfig("cfg3", 10_000, 100_000, 16, "priority+gang+drf+predicates+proportion+nodeorder+binpack"),
+    # cfg3 with hierarchical drf: its 16 queues as 4 departments x 4 teams, unequal weights
+    "cfg3_hdrf": SynthConfig("cfg3_hdrf", 10_000, 100_000, 16, "priority+gang+drf+predicates+proportion+nodeorder+binpack",
+                             hdrf=(4, 4)),
     # configs[3]: 3-tier HyperNode tree (root -> 32 -> 40 each -> ~39 nodes), network-topology-aware weight 10
     # (hypernode-level binpacking of pods without a network topology; topology-constrained jobs are not generated)
     "cfg4": SynthConfig("cfg4", 50_000, 1_000_000, 16,
@@ -335,7 +339,21 @@ def make_snapshot(cfg: SynthConfig | str, seed: Optional[int] = None) -> Snapsho
         _make_topology(s, cfg, rng)
     if cfg.n_besteffort > 0:
         _make_besteffort(s, cfg, np.random.default_rng((cfg.seed if seed is None else seed) + 7919), job_class)
+    if cfg.hdrf is not None:
+        depts, teams = cfg.hdrf
+        hier = [f"root/dept{(q // teams) % depts}/team{q % teams}" for q in range(Q)]
+        wts = [f"1/{1 + (q // teams) % depts}/{1 + 2 * (q % teams)}" for q in range(Q)]
+        s.set_hdrf(hier, wts, total_request(s))
     return s
+
+
+def total_request(s: Snapshot) -> np.ndarray:
+    """JobInfo.TotalRequest [R][J] of a synthetic snapshot: allocated at open + every pending task (BestEffort ones too)."""
+    treq = s.j_allocated.copy()
+    np.add.at(treq.T, s.t_job, s.t_resreq.T)
+    if s.B:
+        np.add.at(treq.T, s.b_job, s.b_resreq.T)
+    return treq
 
 
 def _make_besteffort(s: Snapshot, cfg: SynthConfig, rng, job_class) -> None:

@@ -16,7 +16,7 @@ from typing import Callable, Dict, List, Optional, Sequence
 import numpy as np
 
 from . import abi
-from .api import HyperNode, Node, Pod, PodGroup, Queue
+from .api import BuildQueueWithAnnos, HyperNode, Node, Pod, PodGroup, Queue  # noqa: F401  (util.BuildQueueWithAnnos)
 from .snapshot import PluginOption, SchedulerConf, Snapshot, encode_cluster
 
 
