@@ -11,7 +11,10 @@ package allocategpu
 import "C"
 
 import (
+	"math"
+	"math/rand"
 	"strconv"
+	"time"
 	"unsafe"
 
 	v1 "k8s.io/api/core/v1"
@@ -397,6 +400,40 @@ func (e *session) recordFitError(t int) {
 	job.NodesFitErrors[task.UID] = fe
 }
 
+// setPreemptOptions hands the preempt action's arguments (preempt.go:90-99) to the library, with what its topology-aware
+// reading reads per running task: PodPriority (Spec.Priority, 0 when nil), Status.StartTime, one time.Now() per run and a
+// seed for the offsets that rand.Intn would draw.
+func setPreemptOptions(ssn *framework.Session, e *session) bool {
+	args := framework.GetArgOfActionFromConf(ssn.Configurations, "preempt")
+	topo, workers, pct, minAbs, maxAbs := false, 16, 10, 1, 100
+	args.GetBool(&topo, stockpreempt.EnableTopologyAwarePreemptionKey)
+	args.GetInt(&workers, stockpreempt.TopologyAwarePreemptWorkerNumKey) // accepted and ignored: the dry runs run at once
+	args.GetInt(&pct, stockpreempt.MinCandidateNodesPercentageKey)
+	args.GetInt(&minAbs, stockpreempt.MinCandidateNodesAbsoluteKey)
+	args.GetInt(&maxAbs, stockpreempt.MaxCandidateNodesAbsoluteKey)
+	n := len(e.runTasks)
+	prio, start := make([]int32, n), make([]int64, n)
+	for i, t := range e.runTasks {
+		prio[i] = stockpreempt.PodPriority(t.Pod)
+		start[i] = math.MinInt64 // VC_START_TIME_UNSET
+		if t.Pod.Status.StartTime != nil {
+			start[i] = t.Pod.Status.StartTime.UnixNano()
+		}
+	}
+	opts := C.vc_preempt_options{topology_aware: 0, min_candidate_nodes_percentage: C.int32_t(pct),
+		min_candidate_nodes_absolute: C.int32_t(minAbs), max_candidate_nodes_absolute: C.int32_t(maxAbs),
+		offset_seed: C.uint64_t(rand.Uint64()), now_ns: C.int64_t(time.Now().UnixNano()), n_running: C.int32_t(n),
+		rt_pod_priority: ptrI(prio), rt_start_ns: ptrL(start)}
+	if topo {
+		opts.topology_aware = 1
+	}
+	if rc := C.vc_snapshot_set_preempt_options(cur.snap, &opts); rc != 0 {
+		fail("preempt options")
+		return false
+	}
+	return true
+}
+
 // ---- backfill / preempt / reclaim on the same device session ------------------------------------------------------------
 
 type followUp struct{ name string }
@@ -425,6 +462,10 @@ func (a *followUp) Execute(ssn *framework.Session) {
 	case "backfill":
 		rc = C.vc_backfill_run(cur.snap, &res)
 	case "preempt":
+		if !setPreemptOptions(ssn, e) {
+			runStock(a.name, ssn)
+			return
+		}
 		rc = C.vc_preempt_run(cur.snap, &res)
 	default:
 		rc = C.vc_reclaim_run(cur.snap, &res)

@@ -318,6 +318,31 @@ typedef struct vc_running_tasks {
 } vc_running_tasks;
 #define VC_TASK_PREEMPT_NEVER 1u /* pod.Spec.PreemptionPolicy == Never (preempt.go:437-441, reclaim.go:140-143) */
 
+/* ---- the preempt action's arguments (actions/preempt/preempt.go:50-99) and what its topology-aware reading reads per
+   running task. Defaults (vc_snapshot_set_preempt_options(s, NULL)): topology_aware 0, 10 / 1 / 100.
+   Determinism contract of the topology-aware reading:
+   - predicateNodes are in NodeList order; node.Tasks in ascending running-task index;
+   - the k-th dry run of one vc_preempt_run (k counts from 0 the preemptors that reach findCandidates with at least one
+     predicate node) starts at offset = splitmix64(offset_seed + k) % len(predicateNodes), where
+       splitmix64(x): z = x + 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
+                      z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31)   (uint64 arithmetic);
+   - the 16 workers with early cancel read as one: the candidates are the first numCandidates nodes with victims in scan
+     order from the offset, wrapping around; ties of pickOneNodeForPreemption go to the earlier candidate of that order;
+   - a victim without Pod.Status.StartTime starts at now_ns (one time.Now() per run);
+   - topologyAwarePreemptWorkerNum is accepted by the callers and ignored. ---- */
+#define VC_START_TIME_UNSET INT64_MIN /* rt_start_ns: Pod.Status.StartTime == nil */
+typedef struct vc_preempt_options {
+  int32_t topology_aware;                 /* enableTopologyAwarePreemption */
+  int32_t min_candidate_nodes_percentage; /* minCandidateNodesPercentage */
+  int32_t min_candidate_nodes_absolute;   /* minCandidateNodesAbsolute */
+  int32_t max_candidate_nodes_absolute;   /* maxCandidateNodesAbsolute */
+  uint64_t offset_seed;                   /* replaces rand.Intn (see above) */
+  int64_t now_ns;                         /* replaces time.Now() for victims without a StartTime, ns since the epoch */
+  int32_t n_running;                      /* length of the two arrays: vc_preempt_run checks it against vc_running_tasks */
+  const int32_t *rt_pod_priority;         /* [n_running] PodPriority: Pod.Spec.Priority, 0 when nil (not TaskInfo.Priority) */
+  const int64_t *rt_start_ns;             /* [n_running] Pod.Status.StartTime in ns, VC_START_TIME_UNSET when nil */
+} vc_preempt_options;
+
 /* ---- results ----------------------------------------------------------------------- */
 #define VC_OP_ALLOCATE 0 /* Statement.Allocate (framework/statement.go:242-302) */
 #define VC_OP_PIPELINE 1 /* Statement.Pipeline (framework/statement.go:146-200) */
@@ -428,6 +453,11 @@ int vc_snapshot_set_nominated(vc_snapshot *s, const int32_t *nominated_node);
    later uploads until replaced (rt == NULL or n_tasks == 0 clears it). */
 int vc_snapshot_set_running(vc_snapshot *s, const vc_running_tasks *rt, const uint32_t *task_flags);
 
+/* Optional, any time before vc_preempt_run: the preempt action's arguments. Copied (arrays included); NULL restores the
+   defaults, under which the action runs its normal reading. VC_EINVAL: arrays missing with n_running > 0. The reclaim
+   action ignores them. */
+int vc_snapshot_set_preempt_options(vc_snapshot *s, const vc_preempt_options *opts);
+
 /* ONE session across the GPUs of a node (SURVEY §8e), one process per GPU: the exact allocate loop with the node axis cut
    over the CTAs of all ranks. Every rank uploads the same snapshot and runs the same replicated control program; a CTA's
    per-step records (its best (score, node); the publication of a run of placements) are written into EVERY rank's mailbox
@@ -465,8 +495,8 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out);
    network-topology-aware plugin weighs a resource BestEffort pods request ("pods" in hypernode.binpack.resources). */
 int vc_backfill_run(vc_snapshot *s, vc_result **out);
 
-/* The preempt action (actions/preempt/preempt.go:101-283, normalPreempt :333-434; topology-aware preemption is off by
-   default and not built) and the reclaim action (actions/reclaim/reclaim.go:56-258) on the session state the preceding
+/* The preempt action (actions/preempt/preempt.go:101-283, normalPreempt :333-434, or topologyAwarePreempt :475-1015 when
+   vc_preempt_options.topology_aware is set) and the reclaim action (actions/reclaim/reclaim.go:56-258) on the session state the preceding
    actions left (vc_allocate_run, each other). Preemptors are the tasks of vc_tasks that are still Pending.
    Split: per preemptor the device evaluates EVERY node at once — plugin predicates in their preempt reading
    (ssn.PredicateForPreemptAction, framework/session.go:679-697: only unresolvable failures reject a node, the pod-count cap
@@ -479,6 +509,13 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out);
    Result: decisions of kind VC_OP_EVICT (task = running-task index) and VC_OP_PIPELINE (task = vc_tasks index) in
    statement order; one visit per Statement (preempt: per preemptor job, then per intra-job preemptor; reclaim: per job),
    VC_VISIT_COMMIT or VC_VISIT_DISCARD (discarded operations are not reported).
+   Topology-aware reading (vc_preempt_options): per preemptor one device pass runs SelectVictimsOnNode as a dry run on every
+   predicate node at once (victims from the tier votes and ValidateVictims, popped in victim-queue order until
+   SimulateAllocatableFn and the FutureIdle fit hold, then reprieved last-popped first, on proportion's simulated queue
+   state) and one single-block pass keeps the first numCandidates successes from the offset and picks the winner
+   (SelectCandidate); the winner's victims are evicted in list order, then the preemptor is pipelined. The determinism
+   contract is listed at vc_preempt_options. VC_EINVAL: its arrays do not match vc_running_tasks, or the arguments give a
+   negative numCandidates for a preemptor (the reference panics in make; 0 is kept: no node is ever picked).
    VC_EUNSUPPORTED: BestEffort pending tasks in the session (vc_snapshot_set_backfill), jobs with a network topology,
    feasible-node sampling, PreferNoSchedule taints, the tdm / network-topology-aware plugins. */
 int vc_preempt_run(vc_snapshot *s, vc_result **out);

@@ -130,6 +130,34 @@ def make_wide_case(seed):
     return tc, tiers, tuple(a for a in actions if a != "allocate") or ("preempt",)  # allocate would fill the idle nodes
 
 
+def make_topo_case(seed):
+    """Topology-aware preemption: make_case's clusters with pod priorities and start times (some unset, many equal), pods
+    with and without an index in their names mixed in one job (the victim order then is not a strict weak order),
+    proportion with or without EnabledPredicate, and random candidate-count arguments, offset seeds and clocks.
+    -> (TestCommonStruct, tiers, actions, conf keyword arguments of RegisterSession)."""
+    from volcano_b200 import abi
+    tc, tiers, actions = make_case(seed)
+    rnd = random.Random(seed * 31337 + 5)
+    for p in tc.Pods:
+        if p.node_name and rnd.random() < 0.7:
+            p.start_time = rnd.choice([1, 2, 3]) * 10 ** 9
+        if p.node_name and rnd.random() < 0.3:  # no pod index: util.LessFn falls back to creation time for this pod
+            p.name += "x"
+        if p.node_name and p.priority is None and rnd.random() < 0.2:
+            p.annotations["volcano.sh/task-priority"] = str(rnd.choice([2, 50]))  # TaskInfo.Priority only
+    for tier in tiers:
+        for opt in tier:
+            if opt.name == "proportion" and rnd.random() < 0.3:
+                opt.enabled &= ~abi.VC_EN_PREDICATE
+    if "preempt" not in actions:
+        actions = actions + ("preempt",)
+    args = {"enableTopologyAwarePreemption": True, "topologyAwarePreemptWorkerNum": rnd.choice([1, 16]),
+            "minCandidateNodesPercentage": rnd.choice([0, 10, 50, 100]), "minCandidateNodesAbsolute": rnd.choice([0, 1, 2, 3]),
+            "maxCandidateNodesAbsolute": rnd.choice([1, 2, 100])}
+    conf = {"configurations": {"preempt": args}, "preempt_seed": rnd.getrandbits(64), "now_ns": rnd.randint(0, 4) * 10 ** 9}
+    return tc, tiers, actions, conf
+
+
 def _plugins_and_actions(rnd):
     voters = [n for n in ("conformance", "gang", "priority", "drf", "proportion") if rnd.random() < 0.75]
     scorers = [n for n in ("predicates", "nodeorder", "binpack") if rnd.random() < 0.5]

@@ -261,3 +261,97 @@ extern "C" int eh_apply(const EhApplyArgs *a) {
   EH_TRY(knz.get(a->knz, (size_t)2 * N)); EH_TRY(pod_count.get(a->pod_count, N)); EH_TRY(rt_ev.get(a->rt_evicted, RT));
   return EH_OK;
 }
+
+// ---- k_evict_dryrun / k_evict_select (topology-aware preemption) ---------------------------------------------------
+#include "topo_args.h"
+
+extern "C" int eh_dryrun(const EhTopoArgs *a) {
+  if (!a || !eh_topo_check(*a)) return EH_EINVAL;
+  const int N = a->N, R = a->R, J = a->J, RT = a->RT;
+  const size_t B = (size_t)(RT > 0 ? RT : 1);
+  DevBuf<double> idle, rel, pip, rt_req, j_alloc, j_share;
+  DevBuf<uint32_t> cstat, rt_has, rt_flags, rt_uid, j_rank;
+  DevBuf<int32_t> rt_off, rt_idx, rt_job, rt_prio, rt_pp, j_queue, j_prio, j_min, j_ready, j_pbe, sa, sb, nv;
+  DevBuf<int64_t> rt_podidx, rt_ts, rt_start;
+  DevBuf<uint8_t> rt_ev, sf, sg, ok;
+  DevBuf<long long> key;
+  std::vector<uint32_t> cs(N);
+  for (int n = 0; n < N; ++n) cs[n] = a->pred[n] ? CS_STATIC_OK : 0u;
+  const size_t RN = (size_t)R * N;
+  EH_TRY(idle.put(a->idle, RN)); EH_TRY(rel.put(a->rel, RN)); EH_TRY(pip.put(a->pip, RN)); EH_TRY(cstat.put(cs.data(), N));
+  EH_TRY(rt_off.put(a->rt_off, (size_t)N + 1)); EH_TRY(rt_idx.put(a->rt_idx, RT)); EH_TRY(rt_req.put(a->rt_req, (size_t)R * RT));
+  EH_TRY(rt_has.put(a->rt_has, RT)); EH_TRY(rt_flags.put(a->rt_flags, RT)); EH_TRY(rt_uid.put(a->rt_uid, RT));
+  EH_TRY(rt_job.put(a->rt_job, RT)); EH_TRY(rt_prio.put(a->rt_prio, RT)); EH_TRY(rt_pp.put(a->rt_pod_prio, RT));
+  EH_TRY(rt_podidx.put(a->rt_podidx, RT)); EH_TRY(rt_ts.put(a->rt_ts, RT)); EH_TRY(rt_start.put(a->rt_start, RT));
+  EH_TRY(rt_ev.put(a->rt_evicted, RT));
+  EH_TRY(j_queue.put(a->j_queue, J)); EH_TRY(j_prio.put(a->j_prio, J)); EH_TRY(j_min.put(a->j_min, J));
+  EH_TRY(j_ready.put(a->j_ready, J)); EH_TRY(j_pbe.put(a->j_pbe, J)); EH_TRY(j_rank.put(a->j_rank, J));
+  EH_TRY(j_alloc.put(a->j_alloc, (size_t)R * J)); EH_TRY(j_share.put(a->j_share, J));
+  EH_TRY(sa.put(nullptr, B)); EH_TRY(sb.put(nullptr, B)); EH_TRY(sf.put(nullptr, B)); EH_TRY(sg.put(nullptr, B));
+  EH_TRY(ok.put(nullptr, N)); EH_TRY(nv.put(nullptr, N)); EH_TRY(key.put(nullptr, 4 * (size_t)N));
+  vct::TopoView v;
+  std::memset(&v, 0, sizeof v);
+  v.R = R; v.N = N; v.J = J; v.RT = RT; v.pods_dim = a->pods_dim; v.n_plugins = a->n_plugins;
+  v.task_order_prio = a->task_order_prio;
+  for (int i = 0; i < a->n_plugins; ++i) { v.plugin[i] = a->plugin[i]; v.tier[i] = a->tier[i]; v.enabled[i] = a->enabled[i]; }
+  v.idle = idle.d; v.rel = rel.d; v.pip = pip.d; v.rt_off = rt_off.d; v.rt_idx = rt_idx.d; v.rt_req = rt_req.d;
+  v.rt_has = rt_has.d; v.rt_flags = rt_flags.d; v.rt_uid = rt_uid.d; v.rt_job = rt_job.d; v.rt_prio = rt_prio.d;
+  v.rt_podidx = rt_podidx.d; v.rt_ts = rt_ts.d; v.rt_evicted = rt_ev.d; v.rt_pod_prio = rt_pp.d; v.rt_start = rt_start.d;
+  v.j_queue = j_queue.d; v.j_prio = j_prio.d; v.j_min = j_min.d; v.j_ready = j_ready.d; v.j_pbe = j_pbe.d;
+  v.j_rank = j_rank.d; v.j_alloc = j_alloc.d; v.j_share = j_share.d;
+  for (int d = 0; d < R; ++d) v.total[d] = a->total[d];
+  v.total_has = a->total_has;
+  vct::TopoTask t;
+  eh_topo_task(*a, t);
+  TopoDry s;
+  s.cstat = cstat.d; s.klass = 0; s.a = sa.d; s.b = sb.d; s.f = sf.d; s.g = sg.d; s.ok = ok.d; s.nv = nv.d; s.key = key.d;
+  if (N > 0) {  // the production geometry (vcalloc.cu)
+    k_evict_dryrun<<<(unsigned)((N + 127) / 128), 128>>>(v, t, s);
+    EH_TRY(cudaGetLastError());
+  }
+  EH_TRY(cudaDeviceSynchronize());
+  EH_TRY(ok.get(a->ok, N)); EH_TRY(nv.get(a->nv, N)); EH_TRY(key.get(a->key, 4 * (size_t)N)); EH_TRY(sa.get(a->victims, RT));
+  return EH_OK;
+}
+
+// one k_evict_select launch over per-node dry-run results; words[0..EV_TOPO_SEQ] receive the mapped hand-out
+struct EhSelectArgs {
+  int N, RT;
+  const uint8_t *pred, *ok;        // [N]
+  const int32_t *nv;               // [N]
+  const long long *key;            // [4][N]
+  const int32_t *rt_off, *victims; // [N+1], [RT]
+  unsigned long long seed_k;
+  int pct, min_abs, max_abs, seq;
+  int32_t *words;                  // [EV_TOPO_SEQ + 1]
+};
+
+extern "C" int eh_topo_seq_word() { return EV_TOPO_SEQ; }
+
+extern "C" int eh_select(const EhSelectArgs *a) {
+  if (!a || a->N < 1 || a->RT < 0 || !a->words || a->rt_off[0] != 0 || a->rt_off[a->N] != a->RT) return EH_EINVAL;
+  for (int n = 0; n < a->N; ++n)
+    if (a->rt_off[n + 1] < a->rt_off[n] || (a->ok[n] && (!a->pred[n] || a->nv[n] < 1 || a->nv[n] > a->rt_off[n + 1] - a->rt_off[n])))
+      return EH_EINVAL;
+  const int N = a->N;
+  std::vector<uint32_t> cs(N);
+  for (int n = 0; n < N; ++n) cs[n] = a->pred[n] ? CS_STATIC_OK : 0u;
+  DevBuf<uint32_t> cstat;
+  DevBuf<uint8_t> ok;
+  DevBuf<int32_t> nv, rt_off, victims;
+  DevBuf<long long> key;
+  EH_TRY(cstat.put(cs.data(), N)); EH_TRY(ok.put(a->ok, N)); EH_TRY(nv.put(a->nv, N)); EH_TRY(key.put(a->key, 4 * (size_t)N));
+  EH_TRY(rt_off.put(a->rt_off, (size_t)N + 1)); EH_TRY(victims.put(a->victims, a->RT));
+  Mapped out;
+  EH_TRY(out.alloc(EV_TOPO_SEQ + 1));
+  for (int i = 0; i <= EV_TOPO_SEQ; ++i) out.h[i] = -7;
+  out.h[EV_TOPO_SEQ] = ~a->seq;
+  TopoSelect s;
+  s.cstat = cstat.d; s.klass = 0; s.N = N; s.ok = ok.d; s.nv = nv.d; s.key = key.d; s.rt_off = rt_off.d; s.victims = victims.d;
+  s.seed_k = a->seed_k; s.pct = a->pct; s.min_abs = a->min_abs; s.max_abs = a->max_abs; s.out = out.d; s.seq = a->seq;
+  k_evict_select<<<1, 1024>>>(s);
+  EH_TRY(cudaGetLastError());
+  EH_TRY(cudaDeviceSynchronize());
+  for (int i = 0; i <= EV_TOPO_SEQ; ++i) a->words[i] = reinterpret_cast<volatile int32_t *>(out.h)[i];
+  return EH_OK;
+}

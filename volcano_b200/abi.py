@@ -210,6 +210,16 @@ class vc_running_tasks(C.Structure):
                 ("flags", C.POINTER(C.c_uint32))]
 
 
+VC_START_TIME_UNSET = -(2 ** 63)
+
+
+class vc_preempt_options(C.Structure):
+    _fields_ = [("topology_aware", C.c_int32), ("min_candidate_nodes_percentage", C.c_int32),
+                ("min_candidate_nodes_absolute", C.c_int32), ("max_candidate_nodes_absolute", C.c_int32),
+                ("offset_seed", C.c_uint64), ("now_ns", C.c_int64), ("n_running", C.c_int32),
+                ("rt_pod_priority", _i32p), ("rt_start_ns", _i64p)]
+
+
 class vc_decision(C.Structure):
     _fields_ = [("task", C.c_int32), ("node", C.c_int32), ("kind", C.c_int32), ("visit", C.c_int32),
                 ("score", C.c_double)]
@@ -246,6 +256,7 @@ SYMBOLS = {
     "vc_snapshot_set_backfill": (C.c_int, [_vp, C.c_int32, C.POINTER(vc_tasks)]),
     "vc_snapshot_set_running": (C.c_int, [_vp, C.POINTER(vc_running_tasks), C.POINTER(C.c_uint32)]),
     "vc_snapshot_set_nominated": (C.c_int, [_vp, C.POINTER(C.c_int32)]),
+    "vc_snapshot_set_preempt_options": (C.c_int, [_vp, C.POINTER(vc_preempt_options)]),
     "vc_comm_create": (C.c_int, [_vp, C.c_int, C.c_int, C.c_void_p]),
     "vc_comm_attach": (C.c_int, [_vp, C.c_void_p]),
     "vc_comm_prepare": (C.c_int, [_vp]),

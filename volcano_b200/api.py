@@ -188,6 +188,7 @@ class Pod:
     preemption_policy: str = ""    # pod.Spec.PreemptionPolicy ("Never": the pod never preempts / reclaims)
     priority_class_name: str = ""  # pod.Spec.PriorityClassName (conformance: system-*-critical pods are never evicted)
     nominated_node_name: str = ""  # pod.Status.NominatedNodeName (left by a preemption of an earlier cycle, allocate.go:624-634)
+    start_time: Optional[int] = None  # pod.Status.StartTime in ns since the epoch (None: not started)
 
     def __post_init__(self):
         if not self.uid:

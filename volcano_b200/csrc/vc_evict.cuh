@@ -14,6 +14,7 @@
 // node) and runs in the host control loop (vc_evict.hpp), like the reference's action goroutine.
 #pragma once
 #include "vc_device.cuh"
+#include "vc_topo.hpp"
 
 #define EV_MODE_PREEMPT_INTER 0  // victims: other jobs of the preemptor's queue (preempt.go:198-214)
 #define EV_MODE_PREEMPT_INTRA 1  // victims: the preemptor's own job (preempt.go:252-268)
@@ -395,4 +396,157 @@ __global__ void k_evict_apply(EvictParams p, EvictTask t, int undo) {
     if (d == 63) p.rt_evicted[r] = undo ? 0 : 1;
   }
   if (!undo) pipeline();
+}
+
+// ---- topology-aware preemption (vc_topo.hpp) -----------------------------------------------------------------------
+// k_evict_dryrun: SelectVictimsOnNode as a dry run on every node that passes the preemptor's predicates, one thread per
+// node. Node n's scratch is [rt_off[n], rt_off[n+1]) of four slabs over the running tasks, so a node may run any number
+// of pods; its victims stay in slab a for k_evict_select.
+struct TopoDry {
+  const uint32_t *cstat;  // [C][N]
+  int klass;
+  int32_t *a, *b;         // [RT]
+  uint8_t *f, *g;         // [RT]
+  uint8_t *ok;            // [N] 1 = the node is a candidate
+  int32_t *nv;            // [N] its victim count
+  long long *key;         // [4][N] pickOneNodeForPreemption's scores
+};
+__global__ void __launch_bounds__(128) k_evict_dryrun(vct::TopoView v, vct::TopoTask t, TopoDry s) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= v.N) return;
+  uint8_t ok = 0;
+  if (s.cstat[(size_t)s.klass * v.N + n] & CS_STATIC_OK) {
+    const int o = v.rt_off[n];
+    const vct::TopoResult r = vct::topo_dry_run(v, t, n, s.a + o, s.b + o, s.f + o, s.g + o);
+    ok = (uint8_t)r.ok;
+    s.nv[n] = r.nv;
+    for (int k = 0; k < 4; ++k) s.key[(size_t)k * v.N + n] = r.key[k];
+  }
+  s.ok[n] = ok;
+}
+
+// k_evict_select: one block. The predicate nodes' positions (NodeList order) and the candidates' ranks in scan order
+// from the offset come from one block scan; the first numCandidates candidates compete on the four scores, ties going to
+// the lower rank. The hand-out goes to mapped pinned memory: [0] node (-1: none), [1] victim count, [2]
+// len(predicateNodes), [3] 1 when the victims do not fit the hand-out, [4..] victims in list order; the last store is
+// `seq` into [EV_TOPO_SEQ].
+#define EV_TOPO_SEQ (4 + EV_MAX_VICTIMS)
+struct TopoSelect {
+  const uint32_t *cstat;
+  int klass, N;
+  const uint8_t *ok;
+  const int32_t *nv;
+  const long long *key;
+  const int32_t *rt_off, *victims;  // victims: slab a of k_evict_dryrun
+  unsigned long long seed_k;        // offset_seed + k
+  int pct, min_abs, max_abs;
+  int32_t *out;
+  int seq;
+};
+__global__ void __launch_bounds__(1024) k_evict_select(TopoSelect s) {
+  __shared__ int sp[1024], ss[1024];
+  __shared__ long long wk[32][4];
+  __shared__ long long wr[32];
+  __shared__ int wn[32];
+  __shared__ int s_off;
+  const int tid = threadIdx.x, nt = blockDim.x, N = s.N;
+  const int chunk = (N + nt - 1) / nt;
+  const int lo = min(N, tid * chunk), hi = min(N, lo + chunk);
+  auto pred = [&](int n) { return (s.cstat[(size_t)s.klass * N + n] & CS_STATIC_OK) != 0; };
+  int cp = 0, cs = 0;
+  for (int n = lo; n < hi; ++n)
+    if (pred(n)) { cp += 1; cs += s.ok[n]; }
+  sp[tid] = cp; ss[tid] = cs;
+  if (tid == 0) s_off = 0;
+  __syncthreads();
+  for (int o = 1; o < nt; o <<= 1) {  // inclusive scan
+    const int a = tid >= o ? sp[tid - o] : 0, b = tid >= o ? ss[tid - o] : 0;
+    __syncthreads();
+    sp[tid] += a; ss[tid] += b;
+    __syncthreads();
+  }
+  const long long P = sp[nt - 1], S = ss[nt - 1];
+  const long long pbase = sp[tid] - cp, sbase = ss[tid] - cs;
+  volatile int32_t *out = s.out;
+  if (P == 0) {
+    if (tid == 0) {
+      out[0] = -1; out[1] = 0; out[2] = 0; out[3] = 0;
+      __threadfence_system();
+      out[EV_TOPO_SEQ] = s.seq;
+    }
+    return;
+  }
+  const long long offset = (long long)(vct::splitmix64(s.seed_k) % (unsigned long long)P);
+  const long long numc = vct::num_candidates(P, s.pct, s.min_abs, s.max_abs);
+  if (numc < 0) {
+    if (tid == 0) {
+      out[0] = -1; out[1] = 0; out[2] = (int32_t)P; out[3] = 2;
+      __threadfence_system();
+      out[EV_TOPO_SEQ] = s.seq;
+    }
+    return;
+  }
+  int before = 0;  // candidates whose position is below the offset
+  {
+    long long pi = pbase;
+    for (int n = lo; n < hi; ++n)
+      if (pred(n)) { if (s.ok[n] && pi < offset) before += 1; pi += 1; }
+  }
+  if (before) atomicAdd(&s_off, before);
+  __syncthreads();
+  const long long S_off = s_off;
+  long long bk[4] = {0, 0, 0, 0}, br = -1;
+  int bn = -1;
+  {
+    long long pi = pbase, si = sbase;
+    for (int n = lo; n < hi; ++n) {
+      if (!pred(n)) continue;
+      if (s.ok[n]) {
+        const long long rank = pi >= offset ? si - S_off : (S - S_off) + si;
+        if (rank < numc) {
+          long long k[4];
+          for (int x = 0; x < 4; ++x) k[x] = s.key[(size_t)x * N + n];
+          if (vct::topo_better(k, rank, bk, br)) { for (int x = 0; x < 4; ++x) bk[x] = k[x]; br = rank; bn = n; }
+        }
+        si += 1;
+      }
+      pi += 1;
+    }
+  }
+  const int lane = tid & 31, warp = tid >> 5;
+  for (int o = 16; o; o >>= 1) {
+    long long ok[4];
+    for (int x = 0; x < 4; ++x) ok[x] = __shfl_xor_sync(0xffffffffu, bk[x], o);
+    const long long orr = __shfl_xor_sync(0xffffffffu, br, o);
+    const int on = __shfl_xor_sync(0xffffffffu, bn, o);
+    if (vct::topo_better(ok, orr, bk, br)) { for (int x = 0; x < 4; ++x) bk[x] = ok[x]; br = orr; bn = on; }
+  }
+  if (lane == 0) { for (int x = 0; x < 4; ++x) wk[warp][x] = bk[x]; wr[warp] = br; wn[warp] = bn; }
+  __syncthreads();
+  if (warp == 0) {
+    const int nw = (nt + 31) >> 5;
+    for (int x = 0; x < 4; ++x) bk[x] = lane < nw ? wk[lane][x] : 0;
+    br = lane < nw ? wr[lane] : -1;
+    bn = lane < nw ? wn[lane] : -1;
+    for (int o = 16; o; o >>= 1) {
+      long long ok[4];
+      for (int x = 0; x < 4; ++x) ok[x] = __shfl_xor_sync(0xffffffffu, bk[x], o);
+      const long long orr = __shfl_xor_sync(0xffffffffu, br, o);
+      const int on = __shfl_xor_sync(0xffffffffu, bn, o);
+      if (vct::topo_better(ok, orr, bk, br)) { for (int x = 0; x < 4; ++x) bk[x] = ok[x]; br = orr; bn = on; }
+    }
+    if (lane == 0) wn[0] = bn;
+  }
+  __syncthreads();
+  const int w = wn[0];
+  const int nv = w >= 0 ? s.nv[w] : 0;
+  if (w >= 0)
+    for (int i = tid; i < min(nv, EV_MAX_VICTIMS); i += nt) out[4 + i] = s.victims[s.rt_off[w] + i];
+  if (tid == 0) { out[0] = w; out[1] = nv; out[2] = (int32_t)P; out[3] = nv > EV_MAX_VICTIMS ? 1 : 0; }
+  __threadfence_system();
+  __syncthreads();
+  if (tid == 0) {
+    __threadfence_system();
+    out[EV_TOPO_SEQ] = s.seq;
+  }
 }

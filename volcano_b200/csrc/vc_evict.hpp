@@ -82,6 +82,9 @@ struct Ranker {
   std::function<int(int *node)> next;
   std::function<int(int t, int node, const std::vector<int> &victims)> apply;
   std::function<int(int t, int node, const std::vector<int> &victims)> revert;  // the inverse, for a discarded statement
+  // topology-aware preemption: dry runs on every predicate node and SelectCandidate for preemptor `t`; -> the chosen node
+  // (-1: no candidate) and its victims in eviction order. Set only when the action runs that reading.
+  std::function<int(int t, int mode, int *node, std::vector<int> *victims)> topo;
 };
 
 struct EvictSession {
@@ -496,7 +499,20 @@ struct EvictSession {
     *assigned = false;
     if ((*t_flags)[t] & VC_TASK_PREEMPT_NEVER) return VC_OK;  // preempt.go:436-441 (reclaim checks it in its own loop)
     const int pj = k->t_job[t], q = k->j_queue[pj];
-    int rc = rk.begin(t, mode);
+    int rc;
+    if (rk.topo && mode != 2) {  // topologyAwarePreempt, preempt.go:475-520
+      int n = -1;
+      std::vector<int> victims;
+      if ((rc = rk.topo(t, mode, &n, &victims)) || n < 0) return rc;
+      std::vector<EvictOp> node_stmt;
+      for (int v : victims) evict(node_stmt, v);  // prepareCandidate
+      pipeline(node_stmt, t, n);
+      stmt.insert(stmt.end(), node_stmt.begin(), node_stmt.end());
+      if ((rc = rk.apply(t, n, victims))) return rc;
+      *assigned = true;
+      return VC_OK;
+    }
+    rc = rk.begin(t, mode);
     if (rc) return rc;
     for (;;) {
       int n = -1;

@@ -278,6 +278,13 @@ struct vc_snapshot {
   void *d_ev = nullptr;            // device slab: running-task table + per-preemptor scratch
   size_t d_ev_bytes = 0;
   int32_t *h_ev = nullptr;         // mapped pinned: [0..EV_PICK_K) picked nodes, [EV_CMD_OFF..] apply command
+  // preempt's arguments (vc_snapshot_set_preempt_options) and the topology-aware reading's device state
+  vc_preempt_options popt{0, 10, 1, 100, 0, 0, 0, nullptr, nullptr};
+  std::vector<int32_t> popt_prio;
+  std::vector<int64_t> popt_start;
+  void *d_topo = nullptr;          // device slab: running-task keys, drf job state, per-node dry-run results and scratch
+  size_t d_topo_bytes = 0;
+  int32_t *h_topo = nullptr;       // mapped pinned: k_evict_select's hand-out, EV_TOPO_SEQ = its sequence word
   // ---- one session across the GPUs of a node (vc_comm_create / vc_comm_attach) ----
   int world = 1, rank = 0;
   int n_cta_total = 0;             // CTAs of all ranks (the exchange); n_cta stays this rank's grid
@@ -501,9 +508,9 @@ void vc_snapshot_destroy(vc_snapshot *s) {
     if (r != s->rank && s->peer_comm[r]) cudaIpcCloseMemHandle(s->peer_comm[r]);
   if (s->comm) cudaFree(s->comm);
   void *dptrs[] = {s->in.dev, s->cstat, s->w_idle, s->w_used, s->w_pip, s->w_kreq, s->w_knz, s->w_pod_count,
-                   s->rep_i32, s->rep_f64, s->rep_heap, s->rep_hn_used, s->rep_placed, s->d_job_alloc, s->hn_score, s->mbox, s->ring, s->d_score_log, s->d_prof, s->d_wait, s->d_dbg, s->d_nominated, s->d_decisions, s->d_visits, s->d_fit, s->d_counters, s->d_bf, s->w_rel, s->d_ev, s->d_hd, s->rep_hd, s->d_hdp};
+                   s->rep_i32, s->rep_f64, s->rep_heap, s->rep_hn_used, s->rep_placed, s->d_job_alloc, s->hn_score, s->mbox, s->ring, s->d_score_log, s->d_prof, s->d_wait, s->d_dbg, s->d_nominated, s->d_decisions, s->d_visits, s->d_fit, s->d_counters, s->d_bf, s->w_rel, s->d_ev, s->d_hd, s->rep_hd, s->d_hdp, s->d_topo};
   for (void *p : dptrs) if (p) cudaFree(p);
-  void *hptrs[] = {s->in.pin, s->h_decisions, s->h_visits, s->h_fit, s->h_counters, s->h_ev, s->delta_pin};
+  void *hptrs[] = {s->in.pin, s->h_decisions, s->h_visits, s->h_fit, s->h_counters, s->h_ev, s->delta_pin, s->h_topo};
   if (s->delta_dev) cudaFree(s->delta_dev);
   for (void *p : hptrs) if (p) cudaFreeHost(p);
   if (s->ev0) cudaEventDestroy(s->ev0);
@@ -1787,6 +1794,22 @@ int vc_snapshot_set_running(vc_snapshot *s, const vc_running_tasks *rt, const ui
   return VC_OK;
 }
 
+int vc_snapshot_set_preempt_options(vc_snapshot *s, const vc_preempt_options *opts) {
+  if (!s) return fail(VC_EINVAL, "null snapshot");
+  if (!opts) {
+    s->popt = vc_preempt_options{0, 10, 1, 100, 0, 0, 0, nullptr, nullptr};
+    s->popt_prio.clear(); s->popt_start.clear();
+    return VC_OK;
+  }
+  if (opts->n_running < 0 || (opts->n_running > 0 && (!opts->rt_pod_priority || !opts->rt_start_ns)))
+    return fail(VC_EINVAL, "preempt options: pod priorities / start times missing");
+  s->popt = *opts;
+  s->popt_prio.assign(opts->rt_pod_priority, opts->rt_pod_priority + opts->n_running);
+  s->popt_start.assign(opts->rt_start_ns, opts->rt_start_ns + opts->n_running);
+  s->popt.rt_pod_priority = nullptr; s->popt.rt_start_ns = nullptr;
+  return VC_OK;
+}
+
 namespace {
 
 // session state of the evicting actions: the opening session plus whatever vc_allocate_run did
@@ -1926,6 +1949,66 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     p.exact_sums = (s->rows_integral && vch::max_abs_integral(s->rt.req.data(), s->rt.req.size(), m1) &&
                     vch::max_abs_integral(k.t_req.data(), k.t_req.size(), m2) && m1 * 4096.0 < 9.0e15) ? 1 : 0;
   }
+  // topology-aware preemption: the dry run's inputs beyond the ranking's, its per-node results and scratch
+  const bool topo_on = !reclaim && s->popt.topology_aware;
+  vct::TopoView tv;
+  std::memset(&tv, 0, sizeof tv);
+  TopoDry tdry;
+  std::memset(&tdry, 0, sizeof tdry);
+  double *d_jalloc = nullptr, *d_jshare = nullptr;
+  if (topo_on) {
+    if (s->popt.n_running != s->rt.n)
+      return fail(VC_EINVAL, "preempt options: %d pod priorities / start times for %d running tasks", s->popt.n_running, s->rt.n);
+    size_t toff = 0;
+    auto ttake = [&](size_t bytes) { size_t o = toff; toff = (toff + bytes + 255) & ~(size_t)255; return o; };
+    const size_t J1 = std::max<size_t>(J, 1);
+    const size_t t_rank = ttake(J1 * 4), t_pbe = ttake(J1 * 4), t_jalloc = ttake(R * J1 * 8), t_jshare = ttake(J1 * 8),
+                 t_podidx = ttake(B * 8), t_ts = ttake(B * 8), t_uid = ttake(B * 4), t_has = ttake(B * 4), t_pprio = ttake(B * 4),
+                 t_start = ttake(B * 8), t_a = ttake(B * 4), t_b = ttake(B * 4), t_f = ttake(B), t_g = ttake(B), t_ok = ttake(N),
+                 t_nv = ttake(N * 4), t_key = ttake(4 * N * 8);
+    if (toff > s->d_topo_bytes) {
+      if (s->d_topo) cudaFree(s->d_topo);
+      s->d_topo = nullptr;
+      CUDA_TRY(cudaMalloc(&s->d_topo, toff));
+      s->d_topo_bytes = toff;
+    }
+    if (!s->h_topo) CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&s->h_topo), (EV_TOPO_SEQ + 1) * 4, cudaHostAllocMapped));
+    unsigned char *tb = reinterpret_cast<unsigned char *>(s->d_topo);
+    auto up = [&](size_t o, const void *src, size_t bytes) -> int {
+      if (bytes) CUDA_TRY(cudaMemcpyAsync(tb + o, src, bytes, cudaMemcpyHostToDevice, s->stream));
+      return VC_OK;
+    };
+    const vch::RunningTasks &b = s->rt;
+    std::vector<uint32_t> rt_has(b.has);
+    for (uint32_t &h : rt_has) h &= ~(VC_RES_HAS_ANY | 3u);
+    if ((rc = up(t_rank, k.j_rank.data(), J * 4)) || (rc = up(t_pbe, k.j_pbe.data(), J * 4)) ||
+        (rc = up(t_podidx, b.podidx.data(), b.n * 8)) || (rc = up(t_ts, b.ts.data(), b.n * 8)) ||
+        (rc = up(t_uid, b.uid.data(), b.n * 4)) || (rc = up(t_has, rt_has.data(), b.n * 4)) ||
+        (rc = up(t_pprio, s->popt_prio.data(), b.n * 4)) || (rc = up(t_start, s->popt_start.data(), b.n * 8)))
+      return rc;
+    tv.R = (int)R; tv.N = (int)N; tv.J = (int)J; tv.RT = (int)B; tv.pods_dim = D.pods_dim;
+    tv.n_plugins = s->conf.n_plugins;
+    for (int i = 0; i < s->conf.n_plugins; ++i) {
+      tv.plugin[i] = s->conf.plugins[i].plugin; tv.tier[i] = s->conf.plugins[i].tier; tv.enabled[i] = s->conf.plugins[i].enabled;
+    }
+    tv.task_order_prio = vch::plugin_enabled(s->conf, VC_PLUGIN_PRIORITY, VC_EN_TASK_ORDER) ? 1 : 0;
+    tv.idle = s->w_idle; tv.rel = s->w_rel; tv.pip = s->w_pip;
+    tv.rt_off = p.rt_off; tv.rt_idx = p.rt_idx; tv.rt_req = p.rt_req; tv.rt_flags = p.rt_flags; tv.rt_job = p.rt_job;
+    tv.rt_prio = p.rt_prio; tv.rt_evicted = p.rt_evicted;
+    tv.rt_has = reinterpret_cast<const uint32_t *>(tb + t_has); tv.rt_uid = reinterpret_cast<const uint32_t *>(tb + t_uid);
+    tv.rt_podidx = reinterpret_cast<const int64_t *>(tb + t_podidx); tv.rt_ts = reinterpret_cast<const int64_t *>(tb + t_ts);
+    tv.rt_pod_prio = reinterpret_cast<const int32_t *>(tb + t_pprio); tv.rt_start = reinterpret_cast<const int64_t *>(tb + t_start);
+    tv.j_queue = p.j_queue; tv.j_prio = p.j_prio; tv.j_min = p.j_min; tv.j_ready = p.j_ready;
+    tv.j_pbe = reinterpret_cast<const int32_t *>(tb + t_pbe); tv.j_rank = reinterpret_cast<const uint32_t *>(tb + t_rank);
+    d_jalloc = reinterpret_cast<double *>(tb + t_jalloc); d_jshare = reinterpret_cast<double *>(tb + t_jshare);
+    tv.j_alloc = d_jalloc; tv.j_share = d_jshare;
+    for (size_t d = 0; d < R; ++d) tv.total[d] = e.total[d];
+    tv.total_has = e.total_has;
+    tdry.cstat = s->cstat;
+    tdry.a = reinterpret_cast<int32_t *>(tb + t_a); tdry.b = reinterpret_cast<int32_t *>(tb + t_b);
+    tdry.f = tb + t_f; tdry.g = tb + t_g; tdry.ok = tb + t_ok;
+    tdry.nv = reinterpret_cast<int32_t *>(tb + t_nv); tdry.key = reinterpret_cast<long long *>(tb + t_key);
+  }
   // ReadyTaskNum per job and proportion's "queue above deserved" as the session stands; refreshed after every success
   std::vector<uint8_t> q_over(std::max<size_t>(Q, 1), 0);
   auto refresh_dynamic = [&]() -> int {
@@ -1933,6 +2016,10 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
       q_over[q] = (e.qattr[q].exists && !e.qattr[q].allocated.less_equal_zero(e.qattr[q].deserved, (int)R)) ? 1 : 0;
     if (J) CUDA_TRY(cudaMemcpyAsync(base + o_jready, e.j_ready.data(), J * 4, cudaMemcpyHostToDevice, s->stream));
     if (Q) CUDA_TRY(cudaMemcpyAsync(base + o_qover, q_over.data(), Q, cudaMemcpyHostToDevice, s->stream));
+    if (topo_on && J) {  // the dry run's drf votes and job order read the live allocations and shares
+      CUDA_TRY(cudaMemcpyAsync(d_jalloc, e.j_alloc.data(), R * J * 8, cudaMemcpyHostToDevice, s->stream));
+      CUDA_TRY(cudaMemcpyAsync(d_jshare, e.j_share.data(), J * 8, cudaMemcpyHostToDevice, s->stream));
+    }
     return VC_OK;
   };
   if ((rc = refresh_dynamic())) return rc;
@@ -2067,6 +2154,64 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   };
   rk.apply = [&](int t, int node, const std::vector<int> &v) { return apply_cmd(t, node, v, 0); };
   rk.revert = [&](int t, int node, const std::vector<int> &v) { return apply_cmd(t, node, v, 1); };
+  int topo_k = 0, topo_seq = 0;  // dry runs that met a predicate node (the offset's k) / hand-outs of k_evict_select
+  if (topo_on) {
+    s->h_topo[EV_TOPO_SEQ] = 0;
+    int32_t *d_out = nullptr;
+    CUDA_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_out), s->h_topo, 0));
+    const bool prop_update = vch::plugin_enabled(s->conf, VC_PLUGIN_PROPORTION, VC_EN_PREEMPTABLE) ||
+                             vch::plugin_enabled(s->conf, VC_PLUGIN_PROPORTION, VC_EN_ALLOCATABLE);
+    const bool prop_state = vch::plugin_enabled(s->conf, VC_PLUGIN_PROPORTION, VC_EN_PREDICATE);
+    const bool prop_alloc = vch::plugin_enabled(s->conf, VC_PLUGIN_PROPORTION, VC_EN_ALLOCATABLE);
+    rk.topo = [&, d_out, prop_update, prop_state, prop_alloc](int t, int mode, int *node, std::vector<int> *victims) -> int {
+      *node = -1;
+      victims->clear();
+      if (N == 0) return VC_OK;
+      cur_mode = mode;
+      vct::TopoTask tt;
+      std::memset(&tt, 0, sizeof tt);
+      tt.job = k.t_job[t]; tt.queue = k.j_queue[tt.job]; tt.intra = mode == EV_MODE_PREEMPT_INTRA ? 1 : 0;
+      tt.job_prio = k.j_prio[tt.job]; tt.task_prio = k.t_prio[t];
+      for (size_t d = 0; d < R; ++d) tt.req[d] = k.t_req[d * T + t];
+      tt.has = k.t_has[t] & ~(VC_RES_HAS_ANY | 3u);
+      tt.sim_update = prop_update; tt.sim_state = prop_state; tt.sim_alloc = prop_alloc;
+      const vch::QAttr &qa = e.qattr[tt.queue];  // proportion's PrePredicateFn clones queueOpts when the preemptor is tried
+      tt.q_exists = qa.exists ? 1 : 0;
+      for (size_t d = 0; d < R; ++d) { tt.qalloc.v[d] = qa.allocated.v[d]; tt.qdes[d] = qa.deserved.v[d]; }
+      tt.qalloc.has = qa.allocated.has; tt.qalloc.nil = qa.allocated.nil ? 1 : 0; tt.qdes_has = qa.deserved.has;
+      tt.now_ns = s->popt.now_ns;
+      TopoDry dr = tdry;
+      dr.klass = k.t_class[t];
+      TopoSelect sel;
+      sel.cstat = s->cstat; sel.klass = dr.klass; sel.N = (int)N; sel.ok = dr.ok; sel.nv = dr.nv; sel.key = dr.key;
+      sel.rt_off = p.rt_off; sel.victims = dr.a; sel.seed_k = s->popt.offset_seed + (uint64_t)topo_k;
+      sel.pct = s->popt.min_candidate_nodes_percentage; sel.min_abs = s->popt.min_candidate_nodes_absolute;
+      sel.max_abs = s->popt.max_candidate_nodes_absolute; sel.out = d_out; sel.seq = ++topo_seq;
+      const double tl0 = now_ms();
+      k_evict_dryrun<<<(unsigned)((N + 127) / 128), 128, 0, s->stream>>>(tv, tt, dr);
+      k_evict_select<<<1, 1024, 0, s->stream>>>(sel);
+      launches += 2;
+      CUDA_TRY(cudaGetLastError());
+      t_launch += now_ms() - tl0;
+      const double tl1 = now_ms();
+      volatile int32_t *h = s->h_topo;
+      for (unsigned spins = 0; h[EV_TOPO_SEQ] != sel.seq; ++spins)
+        if ((spins & 0xfffu) == 0xfffu) {
+          const cudaError_t qe = cudaStreamQuery(s->stream);
+          if (qe != cudaSuccess && qe != cudaErrorNotReady) return fail(VC_ECUDA, "evict select: %s", cudaGetErrorString(qe));
+          if (qe == cudaSuccess && h[EV_TOPO_SEQ] != sel.seq) return fail(VC_ECUDA, "evict select: completion word missing");
+        }
+      t_sync += now_ms() - tl1;
+      if (h[2] > 0) topo_k += 1;
+      if (h[3] == 2)
+        return fail(VC_EINVAL, "preempt options: numCandidates < 0 for %d predicate nodes (the reference panics in make)", h[2]);
+      if (h[0] < 0) return VC_OK;
+      if (h[3]) return fail(VC_EUNSUPPORTED, "more than %d victims on one node", EV_MAX_VICTIMS);
+      *node = h[0];
+      for (int i = 0; i < h[1]; ++i) victims->push_back((int)h[4 + i]);
+      return VC_OK;
+    };
+  }
 
   vc_result *r = new vc_result();
   auto emit = [&](int job, const std::vector<vch::EvictOp> &ops, bool commit) {

@@ -62,6 +62,9 @@ class SchedulerConf:
     min_nodes_to_find: int = 100               # options.go:48-51
     min_percentage_nodes_to_find: int = 5
     last_processed_node_index: int = 0         # util.lastProcessedNodeIndex carried over from the previous cycle
+    configurations: Dict[str, Dict[str, object]] = field(default_factory=dict)  # conf.Configuration: action -> arguments
+    preempt_seed: int = 0                      # topology-aware preemption: the offsets' seed (replaces rand.Intn)
+    now_ns: int = 0                            # topology-aware preemption: time.Now() for victims without a StartTime
 
     @staticmethod
     def default() -> "SchedulerConf":
@@ -95,6 +98,44 @@ def _get_bool(args: Dict[str, object], key: str, default: bool) -> bool:
     if s in ("0", "f", "false"):
         return False
     return default
+
+
+@dataclass
+class PreemptArguments:
+    """The preempt action's arguments after parseArguments (actions/preempt/preempt.go:73-99)."""
+    topology_aware: bool = False
+    worker_num: int = 16  # accepted, ignored: the dry runs all run at once
+    min_candidate_nodes_percentage: int = 10
+    min_candidate_nodes_absolute: int = 1
+    max_candidate_nodes_absolute: int = 100
+
+
+def _arg_int(args: Dict[str, object], key: str, default: int) -> int:
+    """framework.Arguments.GetInt (framework/arguments.go:35-52): argv.(int) — any other type keeps the default."""
+    v = args.get(key, default)
+    if not isinstance(v, int) or isinstance(v, bool):
+        return default
+    if not -2 ** 31 <= v < 2 ** 31:
+        raise ValueError(f"{key}={v}: outside the 32-bit range the library takes")
+    return v
+
+
+def _arg_bool(args: Dict[str, object], key: str, default: bool) -> bool:
+    """framework.Arguments.GetBool (framework/arguments.go:78-95): argv.(bool) — any other type keeps the default."""
+    v = args.get(key, default)
+    return v if isinstance(v, bool) else default
+
+
+def preempt_arguments(conf: SchedulerConf) -> PreemptArguments:
+    """framework.GetArgOfActionFromConf(ssn.Configurations, "preempt") read with Arguments.GetBool / GetInt."""
+    a = conf.configurations.get("preempt", {}) or {}
+    d = PreemptArguments()
+    return PreemptArguments(
+        topology_aware=_arg_bool(a, "enableTopologyAwarePreemption", d.topology_aware),
+        worker_num=_arg_int(a, "topologyAwarePreemptWorkerNum", d.worker_num),
+        min_candidate_nodes_percentage=_arg_int(a, "minCandidateNodesPercentage", d.min_candidate_nodes_percentage),
+        min_candidate_nodes_absolute=_arg_int(a, "minCandidateNodesAbsolute", d.min_candidate_nodes_absolute),
+        max_candidate_nodes_absolute=_arg_int(a, "maxCandidateNodesAbsolute", d.max_candidate_nodes_absolute))
 
 
 def build_conf(conf: SchedulerConf, dim_names: Sequence[str], kdim_names: Sequence[str]) -> abi.vc_conf:
@@ -205,6 +246,8 @@ class Snapshot:
         self.N, self.T, self.J, self.Q, self.C, self.NR, self.R, self.K = N, T, J, Q, C_, NR, R, K
         self.B = B  # BestEffort pending tasks (the backfill action's tasks; not part of T)
         self.RT = 0  # tasks that occupy nodes (victim candidates of preempt / reclaim), see set_running
+        self.preempt_args: Optional[PreemptArguments] = None  # the preempt action's arguments when configured
+        self.preempt_seed, self.now_ns = 0, 0
         self.t_flags = np.zeros(T, np.uint32)  # VC_TASK_* per pending task
         self.t_nominated = np.full(T, -1, np.int32)  # node index of Pod.Status.NominatedNodeName per pending task, -1 none
         self.Wl, self.Wt, self.Z, self.pods_dim = Wl, Wt, Z, pods_dim
@@ -360,6 +403,20 @@ class Snapshot:
             _ptr(g("role"), _I32), _ptr(g("priority"), _I32), _ptr(g("pod_index"), _I64),
             _ptr(g("creation_ts"), _I64), _ptr(g("uid_rank"), _U32))
 
+    def preempt_options(self) -> Optional[abi.vc_preempt_options]:
+        """The argument of vc_snapshot_set_preempt_options, or None for the defaults."""
+        pa = getattr(self, "preempt_args", None)
+        if pa is None:
+            return None
+        n = getattr(self, "RT", 0)
+        if n > 0:
+            self.rt_pod_priority = np.ascontiguousarray(getattr(self, "rt_pod_priority", np.zeros(n)), np.int32)
+            self.rt_start_ns = np.ascontiguousarray(getattr(self, "rt_start_ns", np.full(n, abi.VC_START_TIME_UNSET)), np.int64)
+        return abi.vc_preempt_options(
+            1 if pa.topology_aware else 0, pa.min_candidate_nodes_percentage, pa.min_candidate_nodes_absolute,
+            pa.max_candidate_nodes_absolute, self.preempt_seed & (2 ** 64 - 1), self.now_ns, n,
+            _ptr(self.rt_pod_priority if n > 0 else None, _I32), _ptr(self.rt_start_ns if n > 0 else None, _I64))
+
     def set_running(self, n: int):
         """Allocate the node.Tasks table (vc_running_tasks) for n occupying tasks."""
         f8, i4, i8, u4 = np.float64, np.int32, np.int64, np.uint32
@@ -370,6 +427,8 @@ class Snapshot:
         self.rt_resreq = np.zeros((self.R, n), f8); self.rt_req_has = np.zeros(n, u4)
         self.rt_k8s_req = np.zeros((self.K, n), f8); self.rt_k8s_nonzero_req = np.zeros((self.K, n), f8)
         self.rt_flags = np.zeros(n, u4)
+        self.rt_pod_priority = np.zeros(n, i4)  # PodPriority (preempt.go:567-575)
+        self.rt_start_ns = np.full(n, abi.VC_START_TIME_UNSET, i8)
         self.running_task_keys = [""] * n
 
     def running_tasks(self) -> Optional[abi.vc_running_tasks]:
@@ -933,6 +992,9 @@ def encode_cluster(nodes: Sequence[Node], pods: Sequence[Pod], podgroups: Sequen
             except ValueError:
                 pass
         s.rt_priority[r] = prio
+        s.rt_pod_priority[r] = p.priority if p.priority is not None else 0
+        if p.start_time is not None:
+            s.rt_start_ns[r] = p.start_time
         s.rt_pod_index[r] = pod_index_under_task(p.name)
         s.rt_creation_ts[r] = p.creation_ts
         s.rt_resreq[:, r] = v
@@ -1014,6 +1076,9 @@ def encode_cluster(nodes: Sequence[Node], pods: Sequence[Pod], podgroups: Sequen
                 s.q_request_has[qi] |= has
     s.conf = build_conf(conf, dim_names, KDIM_NAMES)
     s.actions = tuple(conf.actions)
+    if conf.configurations.get("preempt"):
+        s.preempt_args = preempt_arguments(conf)
+        s.preempt_seed, s.now_ns = conf.preempt_seed, conf.now_ns
     if hypernodes is not None:
         encode_hypernodes(s, hypernodes, podgroups, job_pods)
     if any(p.hierarchy for tier in conf.tiers for p in tier if p.name == "drf"):

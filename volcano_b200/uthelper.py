@@ -50,6 +50,8 @@ class TestCommonStruct:
     HyperNodes: Optional[List[HyperNode]] = None  # HyperNodesMap of the reference harness
 
     def RegisterSession(self, tiers: Sequence[Sequence[PluginOption]], actions=("allocate",), **conf_kw) -> Snapshot:
+        """conf_kw: fields of SchedulerConf, e.g. configurations={"preempt": {...}} for the reference's
+        RegisterSession(tiers, []conf.Configuration)."""
         self.conf = SchedulerConf(tiers=[list(t) for t in tiers], actions=tuple(actions), **conf_kw)
         self.snap = encode_cluster(self.Nodes, self.Pods, self.PodGroups, self.Queues, self.conf,
                                    tdm_zone_active=self.TdmZoneActive, hypernodes=self.HyperNodes)
