@@ -477,6 +477,9 @@ func (a *followUp) Execute(ssn *framework.Session) {
 		return
 	}
 	defer C.vc_result_free(res)
+	if a.name != "backfill" { // every PredicateNodes call of preempt / reclaim moves the index under sampling
+		lastProcessedNodeIndex = int32(C.vc_result_stats(res).last_processed_node_index)
+	}
 	visits := unsafe.Slice(C.vc_result_visits(res), int(C.vc_result_num_visits(res)))
 	decs := unsafe.Slice(C.vc_result_decisions(res), int(C.vc_result_num_decisions(res)))
 	if a.name == "backfill" {

@@ -516,8 +516,24 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out);
    (SelectCandidate); the winner's victims are evicted in list order, then the preemptor is pipelined. The determinism
    contract is listed at vc_preempt_options. VC_EINVAL: its arrays do not match vc_running_tasks, or the arguments give a
    negative numCandidates for a preemptor (the reference panics in make; 0 is kept: no node is ever picked).
+   Feasible-node sampling (a session where numNodesToFind(N) < N): every PredicateNodes call of both actions follows this
+   determinism contract; without sampling predicateNodes are every passing node in NodeList order and the index is untouched.
+   - the scanned list: a pending task that allocate left a NodesFitErrors entry with node errors (its predicate failed on
+     every node; not a task skipped through TaskHasFitErrors) scans the nodes passing the static predicate in NodeList
+     order (FilterOutUnschedulableAndUnresolvableNodesForTask); any other task scans the NodeList; P is its length;
+   - numNodesToFind comes from P; the scan visits list[(start + i) % P] from start = util.lastProcessedNodeIndex and keeps
+     the first numNodesToFind nodes that pass ssn.PredicateForPreemptAction (the 16 workers read as one); processed is the
+     scan position of the last one kept + 1, or P when fewer pass; the index becomes (start + processed) % P, and an
+     empty list leaves it alone;
+   - the index is one value for the cycle: vc_allocate_run -> vc_preempt_run (both phases, every preemptor that reaches
+     PredicateNodes, failed ones included; PreemptionPolicy Never does not) -> vc_reclaim_run; vc_stats.last_processed_node_index
+     of each result reports it. Before any action of the cycle ran, vc_conf's value is taken as it is, not modulo N;
+   - predicateNodes keep scan order: SortNodes' equal scores go to the lower scan position, reclaim walks scan order, and
+     the topology-aware offset and candidate order count positions in scan order.
    VC_EUNSUPPORTED: BestEffort pending tasks in the session (vc_snapshot_set_backfill), jobs with a network topology,
-   feasible-node sampling, PreferNoSchedule taints, the tdm / network-topology-aware plugins. */
+   PreferNoSchedule taints, the tdm / network-topology-aware plugins; under sampling, enablePredicateErrorCache with a job
+   whose named roles span several (class, request) groups, and min_nodes_to_find below 1 (numNodesToFind of a list can
+   then be 0; a session whose numNodesToFind(N) is 0 is refused too, although allocate runs it without sampling). */
 int vc_preempt_run(vc_snapshot *s, vc_result **out);
 int vc_reclaim_run(vc_snapshot *s, vc_result **out);
 

@@ -158,6 +158,27 @@ def make_topo_case(seed):
     return tc, tiers, actions, conf
 
 
+def make_samp_case(seed):
+    """Feasible-node sampling: make_case's clusters widened to 3-40 nodes (zone labels and selectors make the static
+    verdicts, and so the filtered lists of starving tasks, differ from task to task), percentage-nodes-to-find 34 / 50 /
+    67 with min-nodes-to-find 1, a carried lastProcessedNodeIndex anywhere in [0, 2N], allocate first in most action
+    lists, and the topology-aware reading in a third of the cases. The predicate error cache is off (with it on, sessions
+    whose named roles span several groups are refused). -> (TestCommonStruct, tiers, actions, conf keyword arguments)."""
+    from volcano_b200.api import BuildNode, BuildResourceList
+    rnd = random.Random(seed * 15485863 + 3)
+    topo = rnd.random() < 0.33
+    tc, tiers, actions, conf = make_topo_case(seed) if topo else (*make_case(seed), {})
+    for i in range(len(tc.Nodes), rnd.randint(max(3, len(tc.Nodes)), 40)):
+        labels = {"zone": rnd.choice(["a", "b"])} if rnd.random() < 0.6 else {}
+        tc.Nodes.append(BuildNode(f"n{i}", BuildResourceList(str(rnd.choice([1, 2, 3, 4])), rnd.choice(["4G", "8G", "16G"]),
+                                                               ("pods", str(rnd.choice([3, 6, 20])))), labels))
+    if rnd.random() < 0.8 and "allocate" not in actions:
+        actions = ("allocate",) + tuple(a for a in actions if a != "enqueue")
+    conf.update(percentage_nodes_to_find=rnd.choice([34, 50, 67]), min_nodes_to_find=1,
+                last_processed_node_index=rnd.randint(0, 2 * len(tc.Nodes)), enable_predicate_error_cache=False)
+    return tc, tiers, actions, conf
+
+
 def _plugins_and_actions(rnd):
     voters = [n for n in ("conformance", "gang", "priority", "drf", "proportion") if rnd.random() < 0.75]
     scorers = [n for n in ("predicates", "nodeorder", "binpack") if rnd.random() < 0.5]

@@ -89,10 +89,10 @@ extern "C" int eh_pick_launch(EhPick *s, int big, int mode, int seq, int32_t *wo
   for (int i = 0; i < EV_PICK_K; ++i) s->pick.h[i] = -7;
   s->pick.h[EV_PICK_K] = ~seq;
   if (!big) {
-    if (smem > 48 * 1024) EH_TRY(cudaFuncSetAttribute(k_evict_pick, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_evict_pick<<<1, 1024, smem>>>(p, mode, seq);
+    if (smem > 48 * 1024) EH_TRY(cudaFuncSetAttribute(k_evict_pick<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_evict_pick<false><<<1, 1024, smem>>>(p, mode, seq);
   } else {
-    k_evict_pick_big<<<1, 1024, 0>>>(p, mode, seq);
+    k_evict_pick_big<false><<<1, 1024, 0>>>(p, mode, seq);
   }
   EH_TRY(cudaGetLastError());
   EH_TRY(cudaDeviceSynchronize());
@@ -306,7 +306,7 @@ extern "C" int eh_dryrun(const EhTopoArgs *a) {
   TopoDry s;
   s.cstat = cstat.d; s.klass = 0; s.a = sa.d; s.b = sb.d; s.f = sf.d; s.g = sg.d; s.ok = ok.d; s.nv = nv.d; s.key = key.d;
   if (N > 0) {  // the production geometry (vcalloc.cu)
-    k_evict_dryrun<<<(unsigned)((N + 127) / 128), 128>>>(v, t, s);
+    k_evict_dryrun<false><<<(unsigned)((N + 127) / 128), 128>>>(v, t, s);
     EH_TRY(cudaGetLastError());
   }
   EH_TRY(cudaDeviceSynchronize());
@@ -349,9 +349,39 @@ extern "C" int eh_select(const EhSelectArgs *a) {
   TopoSelect s;
   s.cstat = cstat.d; s.klass = 0; s.N = N; s.ok = ok.d; s.nv = nv.d; s.key = key.d; s.rt_off = rt_off.d; s.victims = victims.d;
   s.seed_k = a->seed_k; s.pct = a->pct; s.min_abs = a->min_abs; s.max_abs = a->max_abs; s.out = out.d; s.seq = a->seq;
-  k_evict_select<<<1, 1024>>>(s);
+  k_evict_select<false><<<1, 1024>>>(s);
   EH_TRY(cudaGetLastError());
   EH_TRY(cudaDeviceSynchronize());
   for (int i = 0; i <= EV_TOPO_SEQ; ++i) a->words[i] = reinterpret_cast<volatile int32_t *>(out.h)[i];
+  return EH_OK;
+}
+
+// ---- k_evict_samp -----------------------------------------------------------------------------------------------------
+// One PredicateNodes call under sampling: static verdicts `pass` of N nodes, the filter flag, vc_conf's three sampling
+// arguments and the index the call starts from. Out: list[0, *cnt) the sampled nodes in scan order, *idx the index left.
+extern "C" int eh_samp(int N, const uint8_t *pass, int filtered, int pct, int min_nodes, int min_pct, int32_t start,
+                       int32_t *list, int32_t *cnt, int32_t *idx) {
+  if (N < 1 || !pass || !list || !cnt || !idx || start < 0) return EH_EINVAL;
+  std::vector<uint32_t> cs(N);
+  for (int n = 0; n < N; ++n) cs[n] = pass[n] ? CS_STATIC_OK : 0u;
+  DevBuf<uint32_t> cstat;
+  DevBuf<int32_t> d_list, words;  // words: [0] count, [1] index
+  EH_TRY(cstat.put(cs.data(), N));
+  std::vector<int32_t> fill(N, -7);
+  EH_TRY(d_list.put(fill.data(), N));
+  const int32_t w0[2] = {-7, start};
+  EH_TRY(words.put(w0, 2));
+  EvictSamp s;
+  s.cstat = cstat.d; s.klass = 0; s.N = N; s.filtered = filtered ? 1 : 0;
+  s.pct = pct; s.min_nodes = min_nodes; s.min_pct = min_pct;
+  s.idx_in = words.d + 1; s.idx_out = words.d + 1; s.list = d_list.d; s.cnt = words.d;
+  k_evict_samp<<<1, 1024>>>(s);
+  EH_TRY(cudaGetLastError());
+  EH_TRY(cudaDeviceSynchronize());
+  int32_t w[2];
+  EH_TRY(words.get(w, 2));
+  EH_TRY(d_list.get(list, N));
+  *cnt = w[0];
+  *idx = w[1];
   return EH_OK;
 }

@@ -14,6 +14,7 @@
 // node) and runs in the host control loop (vc_evict.hpp), like the reference's action goroutine.
 #pragma once
 #include "vc_device.cuh"
+#include "vc_host.hpp"
 #include "vc_topo.hpp"
 
 #define EV_MODE_PREEMPT_INTER 0  // victims: other jobs of the preemptor's queue (preempt.go:198-214)
@@ -61,6 +62,8 @@ struct EvictParams {
   uint8_t *cand;            // [N] 1 = candidate, 2 = tried
   // pick result (mapped pinned memory): EV_PICK_K nodes in the action's order, -1 = no further candidate
   int32_t *pick_node;
+  // feasible-node sampling (k_evict_samp): the sampled nodes in scan order, the only ones the SAMP pick considers
+  const int32_t *samp_list, *samp_cnt;
   // apply command (mapped pinned memory): [0] node, [1] n_victims, [2..] victim running-task ids
   const int32_t *cmd;
 };
@@ -215,19 +218,22 @@ __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) 
 }
 
 // one block: the next EV_PICK_K candidates in the action's node order (preempt: score descending, lowest index first
-// among equals; reclaim: index ascending); the nodes handed out are marked tried. Tournament with incremental repair:
+// among equals; reclaim: index ascending); the nodes handed out are marked tried. SAMP: the candidates are the nodes of
+// k_evict_samp's list and the index is the position in it (scan order). Tournament with incremental repair:
 // every thread keeps the best of its own nodes in registers, every warp its best in shared memory; handing out a node
 // makes ONE thread rescan its nodes and ONE warp refold, the other 31 entries stay. Used when the keys do not fit in shared
 // memory (k_evict_pick below): repairs read the candidate flags and keys from global memory.
 // The last store of the launch is `seq` into pick_node[EV_PICK_K] (system scope): the host polls that word of the mapped
 // buffer instead of paying a stream synchronisation per hand-out.
+template <bool SAMP>
 __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
   __shared__ unsigned long long s_key[32];
   __shared__ int s_node[32];
   __shared__ int s_best;
   __shared__ int s_pick[EV_PICK_K];  // hand-outs, written to the mapped host buffer once at the end (a store to system memory
                                      // per iteration sits on the critical path of the block-wide barriers)
-  const int N = p.d.N;
+  const int N = SAMP ? *p.samp_cnt : p.d.N;  // SAMP: i walks the sampled list, node_of(i) is the node
+  auto node_of = [&](int i) { return SAMP ? p.samp_list[i] : i; };
   if (threadIdx.x < EV_PICK_K) s_pick[threadIdx.x] = -1;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
   auto better_kn = [](unsigned long long ka, int na, unsigned long long kb, int nb) {
@@ -238,8 +244,8 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
   auto rescan = [&](int skip) {
     bk = 0ull; bn = -1;
     for (int n = threadIdx.x; n < N; n += blockDim.x) {
-      if (n == skip || p.cand[n] != 1) continue;
-      const unsigned long long k = mode == EV_MODE_RECLAIM ? 0ull : p.key[n];
+      if (n == skip || p.cand[node_of(n)] != 1) continue;
+      const unsigned long long k = mode == EV_MODE_RECLAIM ? 0ull : p.key[node_of(n)];
       if (bn < 0 || k > bk) { bk = k; bn = n; }  // ascending n per thread: the first of equal keys stays
     }
   };
@@ -266,8 +272,8 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
         if (better_kn(ok, on, gk, gn)) { gk = ok; gn = on; }
       }
       if (lane == 0) {
-        s_pick[it] = gn;
-        if (gn >= 0) p.cand[gn] = 2;
+        s_pick[it] = gn >= 0 ? node_of(gn) : -1;
+        if (gn >= 0) p.cand[node_of(gn)] = 2;
         s_best = gn;
       }
     }
@@ -298,14 +304,16 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
 // EV_PICK_K candidates in order. Phase 2, one warp: a 32-way merge of those sorted lists. Same order as the sequential
 // tournament: key descending, node ascending.
 extern __shared__ unsigned long long ev_pick_cache[];
+template <bool SAMP>
 __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, int seq) {
   __shared__ unsigned long long l_key[32][EV_PICK_K];
   __shared__ int l_node[32][EV_PICK_K];
   __shared__ int s_pick[EV_PICK_K];
-  const int N = p.d.N;
+  const int N = SAMP ? *p.samp_cnt : p.d.N;  // SAMP: n walks the sampled list, node_of(n) is the node
+  auto node_of = [&](int i) { return SAMP ? p.samp_list[i] : i; };
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int n = threadIdx.x; n < N; n += blockDim.x)  // key + 1 (never wraps: see ev_score_key), 0 = not a candidate
-    ev_pick_cache[n] = p.cand[n] == 1 ? (mode == EV_MODE_RECLAIM ? 1ull : p.key[n] + 1ull) : 0ull;
+    ev_pick_cache[n] = p.cand[node_of(n)] == 1 ? (mode == EV_MODE_RECLAIM ? 1ull : p.key[node_of(n)] + 1ull) : 0ull;
   if (threadIdx.x < EV_PICK_K) s_pick[threadIdx.x] = -1;
   __syncwarp();  // a lane only ever reads the entries it wrote
   auto better_kn = [](unsigned long long ka, int na, unsigned long long kb, int nb) {
@@ -352,7 +360,7 @@ __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, in
         if (better_kn(ok, on, gk, gn)) { gk = ok; gn = on; }
       }
       if (gn < 0) break;
-      if (lane == 0) { s_pick[it] = gn; p.cand[gn] = 2; }
+      if (lane == 0) { s_pick[it] = node_of(gn); p.cand[node_of(gn)] = 2; }
       if (cn == gn) hp += 1;
     }
   }
@@ -410,12 +418,19 @@ struct TopoDry {
   uint8_t *ok;            // [N] 1 = the node is a candidate
   int32_t *nv;            // [N] its victim count
   long long *key;         // [4][N] pickOneNodeForPreemption's scores
+  const int32_t *samp_list, *samp_cnt;  // SAMP: thread i runs on the i-th sampled node
 };
+template <bool SAMP>
 __global__ void __launch_bounds__(128) k_evict_dryrun(vct::TopoView v, vct::TopoTask t, TopoDry s) {
-  const int n = blockIdx.x * blockDim.x + threadIdx.x;
-  if (n >= v.N) return;
+  int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (SAMP) {
+    if (n >= *s.samp_cnt) return;
+    n = s.samp_list[n];
+  } else if (n >= v.N) {
+    return;
+  }
   uint8_t ok = 0;
-  if (s.cstat[(size_t)s.klass * v.N + n] & CS_STATIC_OK) {
+  if (SAMP || (s.cstat[(size_t)s.klass * v.N + n] & CS_STATIC_OK)) {
     const int o = v.rt_off[n];
     const vct::TopoResult r = vct::topo_dry_run(v, t, n, s.a + o, s.b + o, s.f + o, s.g + o);
     ok = (uint8_t)r.ok;
@@ -429,7 +444,7 @@ __global__ void __launch_bounds__(128) k_evict_dryrun(vct::TopoView v, vct::Topo
 // from the offset come from one block scan; the first numCandidates candidates compete on the four scores, ties going to
 // the lower rank. The hand-out goes to mapped pinned memory: [0] node (-1: none), [1] victim count, [2]
 // len(predicateNodes), [3] 1 when the victims do not fit the hand-out, [4..] victims in list order; the last store is
-// `seq` into [EV_TOPO_SEQ].
+// `seq` into [EV_TOPO_SEQ]. SAMP: predicateNodes are k_evict_samp's list, positions are list positions (scan order).
 #define EV_TOPO_SEQ (4 + EV_MAX_VICTIMS)
 struct TopoSelect {
   const uint32_t *cstat;
@@ -442,7 +457,9 @@ struct TopoSelect {
   int pct, min_abs, max_abs;
   int32_t *out;
   int seq;
+  const int32_t *samp_list, *samp_cnt;
 };
+template <bool SAMP>
 __global__ void __launch_bounds__(1024) k_evict_select(TopoSelect s) {
   __shared__ int sp[1024], ss[1024];
   __shared__ long long wk[32][4];
@@ -450,12 +467,14 @@ __global__ void __launch_bounds__(1024) k_evict_select(TopoSelect s) {
   __shared__ int wn[32];
   __shared__ int s_off;
   const int tid = threadIdx.x, nt = blockDim.x, N = s.N;
-  const int chunk = (N + nt - 1) / nt;
-  const int lo = min(N, tid * chunk), hi = min(N, lo + chunk);
-  auto pred = [&](int n) { return (s.cstat[(size_t)s.klass * N + n] & CS_STATIC_OK) != 0; };
+  const int D = SAMP ? *s.samp_cnt : N;  // positions n in [0, D), of node node_of(n)
+  auto node_of = [&](int n) { return SAMP ? s.samp_list[n] : n; };
+  const int chunk = (D + nt - 1) / nt;
+  const int lo = min(D, tid * chunk), hi = min(D, lo + chunk);
+  auto pred = [&](int n) { return SAMP || (s.cstat[(size_t)s.klass * N + n] & CS_STATIC_OK) != 0; };
   int cp = 0, cs = 0;
   for (int n = lo; n < hi; ++n)
-    if (pred(n)) { cp += 1; cs += s.ok[n]; }
+    if (pred(n)) { cp += 1; cs += s.ok[node_of(n)]; }
   sp[tid] = cp; ss[tid] = cs;
   if (tid == 0) s_off = 0;
   __syncthreads();
@@ -490,7 +509,7 @@ __global__ void __launch_bounds__(1024) k_evict_select(TopoSelect s) {
   {
     long long pi = pbase;
     for (int n = lo; n < hi; ++n)
-      if (pred(n)) { if (s.ok[n] && pi < offset) before += 1; pi += 1; }
+      if (pred(n)) { if (s.ok[node_of(n)] && pi < offset) before += 1; pi += 1; }
   }
   if (before) atomicAdd(&s_off, before);
   __syncthreads();
@@ -501,12 +520,13 @@ __global__ void __launch_bounds__(1024) k_evict_select(TopoSelect s) {
     long long pi = pbase, si = sbase;
     for (int n = lo; n < hi; ++n) {
       if (!pred(n)) continue;
-      if (s.ok[n]) {
+      const int m = node_of(n);
+      if (s.ok[m]) {
         const long long rank = pi >= offset ? si - S_off : (S - S_off) + si;
         if (rank < numc) {
           long long k[4];
-          for (int x = 0; x < 4; ++x) k[x] = s.key[(size_t)x * N + n];
-          if (vct::topo_better(k, rank, bk, br)) { for (int x = 0; x < 4; ++x) bk[x] = k[x]; br = rank; bn = n; }
+          for (int x = 0; x < 4; ++x) k[x] = s.key[(size_t)x * N + m];
+          if (vct::topo_better(k, rank, bk, br)) { for (int x = 0; x < 4; ++x) bk[x] = k[x]; br = rank; bn = m; }
         }
         si += 1;
       }
@@ -548,5 +568,89 @@ __global__ void __launch_bounds__(1024) k_evict_select(TopoSelect s) {
   if (tid == 0) {
     __threadfence_system();
     out[EV_TOPO_SEQ] = s.seq;
+  }
+}
+
+// ---- feasible-node sampling (util/predicate_helper.go:43-140) -------------------------------------------------------
+// k_evict_samp: PredicateNodes of one preemptor or reclaimer in the single-worker reading, before the pick (normal
+// reading) or the dry runs (topology-aware reading). The scanned list is the NodeList, or with `filtered` (allocate left
+// the task a NodesFitErrors entry with node errors) the nodes that pass the static verdict, in NodeList order
+// (ssn.FilterOutUnschedulableAndUnresolvableNodesForTask); P is its length. The scan visits list[(start + i) % P] and
+// keeps the first numNodesToFind(P) nodes passing the static verdict (ssn.PredicateForPreemptAction). processed is the
+// scan position of the last node kept + 1, or P when fewer pass, and the index becomes (start + processed) % P; an empty
+// list returns early and leaves the index alone. The kept nodes go to list[0, cnt) in scan order. Only the static bit
+// decides the sample: k_evict_rank's necessary conditions prune inside it through the pick.
+// One block, as k_evict_select: every thread owns a contiguous chunk of nodes, a block scan gives the positions in the
+// scanned list and the ranks among the passing nodes; the rotated rank of a passing node counts from the first passing
+// node at or after `start`. idx_in may alias idx_out (read before the first barrier, written after the last).
+struct EvictSamp {
+  const uint32_t *cstat;
+  int klass, N, filtered;
+  int pct, min_nodes, min_pct;  // vc_conf's percentage / minimum node count / minimum percentage to find
+  const int32_t *idx_in;
+  int32_t *idx_out, *list, *cnt;
+};
+__global__ void __launch_bounds__(1024) k_evict_samp(EvictSamp s) {
+  __shared__ int sp[1024], ss[1024];
+  __shared__ int s_start, s_before, s_proc;
+  const int tid = threadIdx.x, nt = blockDim.x, N = s.N;
+  const int chunk = (N + nt - 1) / nt;
+  const int lo = min(N, tid * chunk), hi = min(N, lo + chunk);
+  auto pass = [&](int n) { return (s.cstat[(size_t)s.klass * N + n] & CS_STATIC_OK) != 0; };
+  int cp = 0, cs = 0;
+  for (int n = lo; n < hi; ++n) {
+    const bool ok = pass(n);
+    cp += (ok || !s.filtered) ? 1 : 0;
+    cs += ok ? 1 : 0;
+  }
+  sp[tid] = cp; ss[tid] = cs;
+  if (tid == 0) { s_start = *s.idx_in; s_before = 0; s_proc = -1; }
+  __syncthreads();
+  for (int o = 1; o < nt; o <<= 1) {  // inclusive scan
+    const int a = tid >= o ? sp[tid - o] : 0, b = tid >= o ? ss[tid - o] : 0;
+    __syncthreads();
+    sp[tid] += a; ss[tid] += b;
+    __syncthreads();
+  }
+  const int P = sp[nt - 1], S = ss[nt - 1];
+  if (P == 0) {
+    if (tid == 0) { *s.cnt = 0; *s.idx_out = s_start; }
+    return;
+  }
+  const int start = s_start % P;
+  const int tf = vch::num_feasible_nodes_to_find(P, s.pct, s.min_nodes, s.min_pct);
+  const int M = min(tf, S);
+  int before = 0;  // passing nodes at positions below start
+  {
+    int pi = sp[tid] - cp;
+    for (int n = lo; n < hi; ++n) {
+      const bool ok = pass(n);
+      if (!ok && s.filtered) continue;
+      if (ok && pi < start) before += 1;
+      pi += 1;
+    }
+  }
+  if (before) atomicAdd(&s_before, before);
+  __syncthreads();
+  const int B = s_before;
+  {
+    int pi = sp[tid] - cp, si = ss[tid] - cs;
+    for (int n = lo; n < hi; ++n) {
+      const bool ok = pass(n);
+      if (!ok && s.filtered) continue;
+      if (ok) {
+        const int rank = pi >= start ? si - B : (S - B) + si;
+        if (rank < M) s.list[rank] = n;
+        if (rank == tf - 1) s_proc = (pi - start + P) % P + 1;  // the numNodesToFind-th node found: the scan stops there
+        si += 1;
+      }
+      pi += 1;
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const int processed = s_proc >= 0 ? s_proc : P;
+    *s.cnt = M;
+    *s.idx_out = (int)(((long long)start + processed) % P);
   }
 }

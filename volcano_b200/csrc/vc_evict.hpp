@@ -72,6 +72,25 @@ struct GoPQ {
 
 struct EvictOp { int kind, task, node; };  // VC_OP_EVICT (task = running-task id) / VC_OP_PIPELINE (task = vc_tasks id)
 
+// Per task: 1 when allocate left job.NodesFitErrors[task] with node errors (allocate.go:599-647), the entries
+// ssn.FilterOutUnschedulableAndUnresolvableNodesForTask filters on. Allocate's fit-error list holds, in order, the tasks
+// whose predicate failed on every node (an entry with node errors) and the tasks it skipped through job.TaskHasFitErrors
+// (an entry without any): a task of a named role is skipped once an earlier task of its role has an entry (FitFailedRoles,
+// api/job_info.go:881-902); a task of an unnamed role never is.
+inline std::vector<uint8_t> fit_error_node_kinds(const int32_t *fit, size_t n_fit, const int32_t *t_role,
+                                                 const uint32_t *r_flags, size_t T) {
+  std::vector<uint8_t> out(T, 0);
+  std::vector<uint8_t> failed;  // [role] 1: the role has an entry
+  for (size_t i = 0; i < n_fit; ++i) {
+    const int t = fit[i], r = t_role[t];
+    if ((size_t)r >= failed.size()) failed.resize((size_t)r + 1, 0);
+    if (!(r_flags[r] & VC_ROLE_EMPTY_NAME) && failed[r]) continue;
+    out[t] = 1;
+    failed[r] = 1;
+  }
+  return out;
+}
+
 // The device side as the control loop sees it
 struct Ranker {
   // rank every node for preemptor `t` under `mode`; then next() yields the candidate nodes in the action's order, -1 at the end

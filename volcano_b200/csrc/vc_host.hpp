@@ -195,7 +195,7 @@ inline double go_pow_uint(double x, unsigned n) {
 }
 
 // CalculateNumOfFeasibleNodesToFind, util/scheduler_helper.go:54-73
-inline int32_t num_feasible_nodes_to_find(int32_t num_all, int32_t pct, int32_t min_nodes, int32_t min_pct) {
+VC_HD int32_t num_feasible_nodes_to_find(int32_t num_all, int32_t pct, int32_t min_nodes, int32_t min_pct) {
   if (num_all <= min_nodes || pct >= 100) return num_all;
   int32_t adaptive = pct;
   if (adaptive <= 0) {

@@ -247,6 +247,11 @@ struct vc_snapshot {
   std::vector<vc_decision> last_dec;  // operations of the last vc_allocate_run (kept visits only)
   bool alloc_ran = false, bf_ran = false;
   int last_idx_cur = 0;   // util.lastProcessedNodeIndex as the last action of the cycle left it
+  // the index as the evicting actions read it: vc_conf's value until an action of the cycle moved it (the filtered
+  // lists of preempt / reclaim are shorter than N, so it is not reduced modulo N before they scan)
+  int evict_idx = 0;
+  std::vector<int32_t> last_fit;  // allocate's fit-error list of the last vc_allocate_run
+  std::vector<uint8_t> t_filtered;  // [T] 1: allocate left the task a NodesFitErrors entry with node errors
   int *d_dbg = nullptr;
   std::vector<int32_t> h_nominated;  // [T] node index per task or -1 (vc_snapshot_set_nominated); empty: none
   bool any_nominated = false;
@@ -1293,7 +1298,8 @@ int vc_snapshot_upload(vc_snapshot *s, const vc_nodes *nd, const vc_tasks *tk, c
   tick("integrality scan");
   s->alloc_ran = false; s->bf_ran = false;
   s->last_idx_cur = s->dc.last_idx0;
-  s->last_dec.clear(); s->last_vis.clear();
+  s->evict_idx = s->conf.last_processed_node_index >= 0 ? s->conf.last_processed_node_index : s->dc.last_idx0;
+  s->last_dec.clear(); s->last_vis.clear(); s->last_fit.clear();
   s->es_built = false;
   {  // what the preempt / reclaim actions read of the opening session
     vch::EvictKeep &k = s->ek;
@@ -1438,7 +1444,8 @@ int vc_snapshot_update_nodes(vc_snapshot *s, int32_t n_dirty, const int32_t *nod
   // the session is at its (new) opening state
   s->alloc_ran = false; s->bf_ran = false; s->es_built = false; s->dense_ready = false;
   s->last_idx_cur = s->dc.last_idx0;
-  s->last_dec.clear(); s->last_vis.clear();
+  s->evict_idx = s->conf.last_processed_node_index >= 0 ? s->conf.last_processed_node_index : s->dc.last_idx0;
+  s->last_dec.clear(); s->last_vis.clear(); s->last_fit.clear();
   s->upload_ms = now_ms() - t0;
   s->h2d_bytes = (int64_t)((4 * R + 2 * K) * m * 8 + m * 8);
   return VC_OK;
@@ -1680,6 +1687,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   s->alloc_ran = true; s->bf_ran = false;
   s->last_dec = r->decisions;  // discarded visits carry no operations
   s->last_vis = r->visits;
+  s->last_fit = r->fit_errors;
   s->es_built = false;  // the session state of the evicting actions is rebuilt from this run's operations
   if (s->topo_any) {
     r->job_alloc.resize(J);
@@ -1726,6 +1734,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   r->stats.last_processed_node_index = (s->dc.to_find > 0 || s->any_nominated) ? s->h_counters[4] : s->dc.last_idx0;
   r->stats.commit_kernel = s->fast ? VC_KERNEL_INCREMENTAL : VC_KERNEL_GENERAL;
   s->last_idx_cur = r->stats.last_processed_node_index;
+  s->evict_idx = s->last_idx_cur;
   for (int k = 0; k < 8; ++k) r->stats.prof_cycles[k] = s->h_prof[k];
   r->stats.prof_cycles[6] = s->h_counters[5];  // full sweeps (fast kernel)
   r->stats.prof_cycles[7] = s->h_counters[6];  // incremental steps (fast kernel)
@@ -1817,7 +1826,14 @@ int ensure_evict_session(vc_snapshot *s) {
   const vc_dims &D = s->dims;
   const size_t N = D.n_nodes, T = D.n_tasks, J = D.n_jobs, Q = D.n_queues, R = D.n_dims, K = D.n_kdims, NR = D.n_roles;
   if (s->bf.n > 0 || s->bf_ran) return fail(VC_EUNSUPPORTED, "preempt / reclaim: BestEffort pending tasks in the session");
-  if (s->dc.to_find > 0) return fail(VC_EUNSUPPORTED, "preempt / reclaim: feasible-node sampling");
+  if (s->conf.min_nodes_to_find < 1 && N > 0 &&
+      vch::num_feasible_nodes_to_find((int32_t)N, s->conf.percentage_nodes_to_find, s->conf.min_nodes_to_find,
+                                      s->conf.min_percentage_nodes_to_find) < (int32_t)N)
+    return fail(VC_EUNSUPPORTED, "preempt / reclaim under feasible-node sampling: min-nodes-to-find below 1 (numNodesToFind "
+                                 "of a list can be 0)");
+  if (s->dc.to_find > 0 && s->dc.enable_ecache && !s->all_pure)
+    return fail(VC_EUNSUPPORTED, "preempt / reclaim under feasible-node sampling: enablePredicateErrorCache with a job whose "
+                                 "named roles span several (class, request) groups (the role-keyed cache is not modelled)");
   if (s->dc.soft_active || s->dc.nta_plugin || vch::has_plugin(s->conf, VC_PLUGIN_TDM))
     return fail(VC_EUNSUPPORTED, "preempt / reclaim: PreferNoSchedule taints, network-topology-aware and tdm are outside the path");
   for (uint8_t f : s->h_job_soft)
@@ -1854,6 +1870,7 @@ int ensure_evict_session(vc_snapshot *s) {
     e.on_allocate(j, e.task_res(t), k.t_req.data(), (int)T, t);
   }
   s->last_dec.clear();  // applied (a second evicting action continues from e)
+  s->t_filtered = vch::fit_error_node_kinds(s->last_fit.data(), s->last_fit.size(), k.t_role.data(), k.r_flags.data(), T);
   // device: working rows (left by allocate, or the opening ones), Releasing, the running-task table, scratch
   cudaError_t ce;
   auto ensure = [&](auto *&ptr, size_t bytes) -> cudaError_t {
@@ -1879,7 +1896,8 @@ int ensure_evict_session(vc_snapshot *s) {
   const size_t o_off = take((N + 1) * 4), o_idx = take(B * 4), o_req = take(R * B * 8), o_kreq = take(K * B * 8),
                o_knz = take(K * B * 8), o_flags = take(B * 4), o_job = take(B * 4), o_ev = take(B), o_key = take(N * 8),
                o_cand = take(N), o_prio = take(B * 4), o_jready = take(std::max<size_t>(J, 1) * 4), o_qover = take(std::max<size_t>(Q, 1)),
-               o_key2 = take(N * 8), o_cand2 = take(N);  // second ranking scratch: the preemptor ranked one ahead
+               o_key2 = take(N * 8), o_cand2 = take(N),  // second ranking scratch: the preemptor ranked one ahead
+               o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4);  // k_evict_samp: lists, counts, indexes
   if (off > s->d_ev_bytes) {
     if (s->d_ev) cudaFree(s->d_ev);
     s->d_ev = nullptr;
@@ -1887,7 +1905,7 @@ int ensure_evict_session(vc_snapshot *s) {
     s->d_ev_bytes = off;
   }
   if (!s->h_ev) CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&s->h_ev), (EV_CMD_OFF + 2 + EV_MAX_VICTIMS) * 4, cudaHostAllocMapped));
-  (void)o_key2; (void)o_cand2;
+  (void)o_key2; (void)o_cand2; (void)o_list; (void)o_list2; (void)o_samp;
   unsigned char *base = reinterpret_cast<unsigned char *>(s->d_ev);
   CUDA_TRY(cudaMemsetAsync(base, 0, off, s->stream));
   if (s->rt.n > 0) {
@@ -1929,7 +1947,8 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   const size_t o_off = take((N + 1) * 4), o_idx = take(B * 4), o_req = take(R * B * 8), o_kreq = take(K * B * 8),
                o_knz = take(K * B * 8), o_flags = take(B * 4), o_job = take(B * 4), o_ev = take(B), o_key = take(N * 8),
                o_cand = take(N), o_prio = take(B * 4), o_jready = take(std::max<size_t>(J, 1) * 4), o_qover = take(std::max<size_t>(Q, 1)),
-               o_key2 = take(N * 8), o_cand2 = take(N);  // second ranking scratch: the preemptor ranked one ahead
+               o_key2 = take(N * 8), o_cand2 = take(N),  // second ranking scratch: the preemptor ranked one ahead
+               o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4);  // k_evict_samp: lists, counts, indexes
   unsigned char *base = reinterpret_cast<unsigned char *>(s->d_ev);
   EvictParams p;
   std::memset(&p, 0, sizeof p);
@@ -2029,6 +2048,26 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   p.pick_node = dev_h; p.cmd = dev_h + EV_CMD_OFF;
   int32_t *h_cmd = s->h_ev + EV_CMD_OFF;
   int launches = 0, cur_mode = 0;
+  // Feasible-node sampling: every PredicateNodes call of the action (k_evict_samp) scans from the index the previous one
+  // left, read and written on the device. d_samp[k] is the sampled count of ranking set k and d_samp[2 + k] the index
+  // its call left; d_samp[4] holds the index the action starts from. idx_live names the slot of the last call the action
+  // consumed: a ranking made ahead scans from the preemptor under trial's slot and becomes live only when it is used.
+  const bool samp = s->dc.to_find > 0;
+  int32_t *d_samp = reinterpret_cast<int32_t *>(base + o_samp);
+  int32_t *d_list[2] = {reinterpret_cast<int32_t *>(base + o_list), reinterpret_cast<int32_t *>(base + o_list2)};
+  int idx_live = 2;
+  if (samp) CUDA_TRY(cudaMemcpyAsync(d_samp + 4, &s->evict_idx, 4, cudaMemcpyHostToDevice, s->stream));
+  auto launch_samp = [&](int set, int t) -> int {
+    EvictSamp sa;
+    sa.cstat = s->cstat; sa.klass = k.t_class[t]; sa.N = (int)N; sa.filtered = s->t_filtered[t];
+    sa.pct = s->conf.percentage_nodes_to_find; sa.min_nodes = s->conf.min_nodes_to_find;
+    sa.min_pct = s->conf.min_percentage_nodes_to_find;
+    sa.idx_in = d_samp + 2 + idx_live; sa.idx_out = d_samp + 2 + set; sa.list = d_list[set]; sa.cnt = d_samp + set;
+    k_evict_samp<<<1, 1024, 0, s->stream>>>(sa);
+    launches++;
+    CUDA_TRY(cudaGetLastError());
+    return VC_OK;
+  };
   EvictTask et;
   auto stage = [&](int t, int mode) {
     std::memset(&et, 0, sizeof et);
@@ -2050,7 +2089,9 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   int pick_buf[EV_PICK_K], pick_pos = EV_PICK_K, pick_n = 0;
   // the pick kernel stages the candidates' keys in shared memory when they fit (N * 8 bytes)
   size_t pick_smem = N * 8 <= 200 * 1024 ? N * 8 : 0;
-  if (pick_smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(k_evict_pick, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pick_smem));
+  if (pick_smem > 48 * 1024)
+    CUDA_TRY(cudaFuncSetAttribute(samp ? k_evict_pick<true> : k_evict_pick<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)pick_smem));
   double t_launch = 0.0, t_sync = 0.0;  // host time inside kernel launches / waiting for a hand-out (vc_stats.prof_cycles, us)
   // Two ranking scratch sets (candidate flags, keys, hand-out slots): while the host walks the candidates of one
   // preemptor the device already ranks the one the control loop will most likely try next (rk.hint). Most preemptors fail,
@@ -2064,11 +2105,15 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   int cur = 0, hint_t = -1, hint_mode = 0, pref_t = -1, pref_mode = 0, n_ahead = 0, n_ahead_used = 0;
   unsigned epoch = 0, pref_epoch = 0;
   bool first_pending = false;  // the first hand-out of the preemptor under trial is launched but not consumed yet
-  auto with_set = [&](int k) { EvictParams q = p; q.key = sets[k].key; q.cand = sets[k].cand; q.pick_node = sets[k].d_pick; return q; };
+  auto with_set = [&](int k) {
+    EvictParams q = p;
+    q.key = sets[k].key; q.cand = sets[k].cand; q.pick_node = sets[k].d_pick; q.samp_list = d_list[k]; q.samp_cnt = d_samp + k;
+    return q;
+  };
   auto launch_pick = [&](int k, int mode) -> int {
     sets[k].seq += 1;
-    if (pick_smem) k_evict_pick<<<1, 1024, pick_smem, s->stream>>>(with_set(k), mode, sets[k].seq);
-    else k_evict_pick_big<<<1, 1024, 0, s->stream>>>(with_set(k), mode, sets[k].seq);
+    if (pick_smem) (samp ? k_evict_pick<true> : k_evict_pick<false>)<<<1, 1024, pick_smem, s->stream>>>(with_set(k), mode, sets[k].seq);
+    else (samp ? k_evict_pick_big<true> : k_evict_pick_big<false>)<<<1, 1024, 0, s->stream>>>(with_set(k), mode, sets[k].seq);
     launches++;
     CUDA_TRY(cudaGetLastError());
     return VC_OK;
@@ -2080,7 +2125,8 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     else k_evict_rank<16, VC_MAX_DIMS><<<(unsigned)((N * 16 + 255) / 256), 256, 0, s->stream>>>(with_set(k), et);
     launches++;
     CUDA_TRY(cudaGetLastError());
-    const int rc2 = launch_pick(k, mode);
+    int rc2 = samp ? launch_samp(k, t) : VC_OK;
+    if (!rc2) rc2 = launch_pick(k, mode);
     t_launch += now_ms() - tl0;
     return rc2;
   };
@@ -2097,6 +2143,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     } else if ((rc2 = launch_rank_pick(cur, t, mode))) {
       return rc2;
     }
+    idx_live = cur;  // this preemptor's PredicateNodes is the one the action consumes
     pref_t = -1;
     first_pending = true;
     if (hint_t >= 0 && hint_t != t) {
@@ -2182,14 +2229,21 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
       tt.now_ns = s->popt.now_ns;
       TopoDry dr = tdry;
       dr.klass = k.t_class[t];
+      dr.samp_list = d_list[0]; dr.samp_cnt = d_samp;
       TopoSelect sel;
       sel.cstat = s->cstat; sel.klass = dr.klass; sel.N = (int)N; sel.ok = dr.ok; sel.nv = dr.nv; sel.key = dr.key;
       sel.rt_off = p.rt_off; sel.victims = dr.a; sel.seed_k = s->popt.offset_seed + (uint64_t)topo_k;
       sel.pct = s->popt.min_candidate_nodes_percentage; sel.min_abs = s->popt.min_candidate_nodes_absolute;
       sel.max_abs = s->popt.max_candidate_nodes_absolute; sel.out = d_out; sel.seq = ++topo_seq;
+      sel.samp_list = dr.samp_list; sel.samp_cnt = dr.samp_cnt;
       const double tl0 = now_ms();
-      k_evict_dryrun<<<(unsigned)((N + 127) / 128), 128, 0, s->stream>>>(tv, tt, dr);
-      k_evict_select<<<1, 1024, 0, s->stream>>>(sel);
+      if (samp) {
+        const int rc2 = launch_samp(0, t);
+        if (rc2) return rc2;
+        idx_live = 0;
+      }
+      (samp ? k_evict_dryrun<true> : k_evict_dryrun<false>)<<<(unsigned)((N + 127) / 128), 128, 0, s->stream>>>(tv, tt, dr);
+      (samp ? k_evict_select<true> : k_evict_select<false>)<<<1, 1024, 0, s->stream>>>(sel);
       launches += 2;
       CUDA_TRY(cudaGetLastError());
       t_launch += now_ms() - tl0;
@@ -2329,6 +2383,13 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
       }
     }
   }
+  if (samp) {  // the index the last PredicateNodes call left, carried into the next action
+    cudaError_t ce = cudaMemcpyAsync(&s->evict_idx, d_samp + 2 + idx_live, 4, cudaMemcpyDeviceToHost, s->stream);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s->stream);
+    if (ce != cudaSuccess) return bail(fail(VC_ECUDA, "evict index: %s", cudaGetErrorString(ce)));
+    s->last_idx_cur = s->evict_idx;
+  }
+  r->stats.last_processed_node_index = samp ? s->evict_idx : s->last_idx_cur;
   r->stats.total_ms = now_ms() - t0;
   r->stats.commit_ms = r->stats.total_ms;
   r->stats.kernel_launches = launches;
@@ -2569,6 +2630,7 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
                     "(republisher, summed) %lld cycles\n", h_prof[8], h_prof[9]);
   s->bf_ran = true;
   if (s->dc.to_find > 0) s->last_idx_cur = h_last;
+  s->evict_idx = s->last_idx_cur;
   r->stats.last_processed_node_index = s->last_idx_cur;
 
   // ---- 5. the result: one visit per job in pick order ----
