@@ -444,7 +444,8 @@ int vc_snapshot_set_backfill(vc_snapshot *s, int32_t n_tasks, const vc_tasks *ta
    cycle) as node indices, [vc_dims.n_tasks], -1 = none or a node that is not in the session. allocate tries such a node first
    (actions/allocate/allocate.go:624-634): if InitResreq <= its FutureIdle, ph.PredicateNodes runs on that one node, and a pass
    makes it the task's only candidate. NULL clears the list. Sessions that carry a nominated task run on the general commit
-   kernel; vc_preempt_run / vc_reclaim_run refuse them (taskEligibleToPreempt's nominated-node rules, preempt.go:436-470, are
+   kernel. vc_reclaim_run runs them: reclaim never reads the nominated node (it checks PreemptionPolicy only,
+   reclaim.go:140-143). vc_preempt_run refuses them (taskEligibleToPreempt's nominated-node rules, preempt.go:436-470, are
    not modelled). The list is copied and stays in effect for later uploads until replaced. */
 int vc_snapshot_set_nominated(vc_snapshot *s, const int32_t *nominated_node);
 
@@ -530,8 +531,11 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out);
      of each result reports it. Before any action of the cycle ran, vc_conf's value is taken as it is, not modulo N;
    - predicateNodes keep scan order: SortNodes' equal scores go to the lower scan position, reclaim walks scan order, and
      the topology-aware offset and candidate order count positions in scan order.
+   PreferNoSchedule taints under TaintToleration's batch score order preempt's normal reading: the count of intolerable
+   ones is normalised by its maximum over predicateNodes (every node passing the static predicate, or under sampling the
+   sampled list), candidates or not; reclaim and the topology-aware reading do not score nodes.
    VC_EUNSUPPORTED: BestEffort pending tasks in the session (vc_snapshot_set_backfill), jobs with a network topology,
-   PreferNoSchedule taints, the tdm / network-topology-aware plugins; under sampling, enablePredicateErrorCache with a job
+   the tdm / network-topology-aware plugins; under sampling, enablePredicateErrorCache with a job
    whose named roles span several (class, request) groups, and min_nodes_to_find below 1 (numNodesToFind of a list can
    then be 0; a session whose numNodesToFind(N) is 0 is refused too, although allocate runs it without sampling). */
 int vc_preempt_run(vc_snapshot *s, vc_result **out);

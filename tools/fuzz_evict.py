@@ -179,6 +179,45 @@ def make_samp_case(seed):
     return tc, tiers, actions, conf
 
 
+def make_soft_case(seed):
+    """PreferNoSchedule taints: make_case's clusters widened to 3-40 nodes, random PreferNoSchedule and NoSchedule taints
+    on the nodes and tolerations (either effect, or every effect) on the pods, nodeorder always on with
+    tainttoleration.weight 0 or 3 (the other scorers as make_case draws them), feasible-node sampling in half the cases
+    and the topology-aware reading in a third. -> (TestCommonStruct, tiers, actions, conf keyword arguments)."""
+    from volcano_b200.api import Taint, Toleration
+    rnd = random.Random(seed * 2750159 + 13)
+    topo = rnd.random() < 0.33
+    tc, tiers, actions, conf = make_topo_case(seed) if topo else (*make_case(seed), {})
+    for i in range(len(tc.Nodes), rnd.randint(max(3, len(tc.Nodes)), 40)):
+        labels = {"zone": rnd.choice(["a", "b"])} if rnd.random() < 0.4 else {}
+        tc.Nodes.append(BuildNode(f"n{i}", BuildResourceList(str(rnd.choice([1, 2, 3, 4])), rnd.choice(["4G", "8G", "16G"]),
+                                                               ("pods", str(rnd.choice([3, 6, 20])))), labels))
+    keys = ["s0", "s1", "s2", "s3"]
+    for n in tc.Nodes:
+        n.taints = [Taint(k, "", "PreferNoSchedule") for k in keys if rnd.random() < 0.3]
+        if rnd.random() < 0.1:
+            n.taints.append(Taint("h0", "", "NoSchedule"))
+    for p in tc.Pods:
+        if not p.node_name and rnd.random() < 0.4:
+            p.tolerations = [Toleration(rnd.choice(keys + ["h0"]), "Exists", "", rnd.choice(["", "PreferNoSchedule", "NoSchedule"]))
+                             for _ in range(rnd.randint(1, 2))]
+    weight = rnd.choice([0, 3])
+    opts = [o for t in tiers for o in t]
+    no = next((o for o in opts if o.name == "nodeorder"), None)
+    if no is None:
+        no = PluginOption.defaults("nodeorder")
+        tiers[-1].append(no)
+    no.arguments["tainttoleration.weight"] = weight
+    if not any(o.name == "predicates" for o in opts) and rnd.random() < 0.7:  # NoSchedule taints reject nodes only here
+        tiers[-1].append(PluginOption.defaults("predicates"))
+    if "preempt" not in actions:
+        actions = actions + ("preempt",)
+    if rnd.random() < 0.5:
+        conf.update(percentage_nodes_to_find=rnd.choice([34, 50, 67]), min_nodes_to_find=1,
+                    last_processed_node_index=rnd.randint(0, 2 * len(tc.Nodes)), enable_predicate_error_cache=False)
+    return tc, tiers, actions, conf
+
+
 def _plugins_and_actions(rnd):
     voters = [n for n in ("conformance", "gang", "priority", "drf", "proportion") if rnd.random() < 0.75]
     scorers = [n for n in ("predicates", "nodeorder", "binpack") if rnd.random() < 0.5]

@@ -131,7 +131,83 @@ struct EhRankArgs {
   unsigned long long *key;  // [N]
 };
 
-extern "C" int eh_rank(const EhRankArgs *a) {
+// The SOFT chain of preempt's normal reading (eh_soft_chain): k_evict_rank<.., true>, k_evict_samp<true> under sampling,
+// then pick launches until the candidates run out. TaintToleration's batch score (weight w_taint) is the only scorer;
+// the soft-taint counts are bits 8..15 of the rank arguments' cstat.
+struct EhSoftArgs {
+  int w_taint;
+  int samp, filtered, pct, min_nodes, min_pct, start;  // samp = 1: one PredicateNodes call between rank and pick
+  int big;                                              // 1: k_evict_pick_big, else k_evict_pick
+  unsigned long long seq, stale;  // the ranking's tag; the reduction word before the launches (an earlier ranking's)
+  int32_t *order;                 // [N] the nodes handed out, in order
+  int32_t *n_order;
+  unsigned long long *word;       // the reduction word after the launches
+};
+
+static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx);
+
+extern "C" int eh_rank(const EhRankArgs *a) { return rank_run(a, nullptr); }
+
+extern "C" int eh_soft_chain(const EhRankArgs *a, const EhSoftArgs *sx) {
+  if (!a || !sx || !sx->order || !sx->n_order || !sx->word || a->N < 1 || a->mode == EV_MODE_RECLAIM) return EH_EINVAL;
+  if ((sx->samp != 0 && sx->samp != 1) || (sx->big != 0 && sx->big != 1) || sx->start < 0) return EH_EINVAL;
+  if (!sx->big && a->N > eh_pick_smem_max_nodes()) return EH_EINVAL;
+  return rank_run(a, sx);
+}
+
+// p / t as rank_run built them (device rows staged, cand / key allocated); rank_run's buffers outlive the call
+static int soft_chain(const EhRankArgs *a, const EhSoftArgs &sx, EvictParams p, const EvictTask &t) {
+  const int N = a->N;
+  p.c.batch_any = 1; p.c.taint_batch = 1; p.c.w_taint = sx.w_taint;
+  DevBuf<unsigned long long> word;
+  DevBuf<int32_t> list, words;  // words: [0] sampled count, [1] index
+  EH_TRY(word.put(&sx.stale, 1));
+  EH_TRY(list.put(nullptr, N));
+  const int32_t w0[2] = {0, sx.start};
+  EH_TRY(words.put(w0, 2));
+  p.soft_word = word.d; p.soft_seq = sx.seq; p.soft_klass = 0; p.soft_reduce = sx.samp ? 0 : 1;
+  p.samp_list = list.d; p.samp_cnt = words.d;
+  if (a->R <= 8) k_evict_rank<16, 8, true><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);
+  else k_evict_rank<16, VC_MAX_DIMS, true><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);
+  EH_TRY(cudaGetLastError());
+  if (sx.samp) {
+    EvictSamp s;
+    s.cstat = p.cstat; s.klass = 0; s.N = N; s.filtered = sx.filtered ? 1 : 0;
+    s.pct = sx.pct; s.min_nodes = sx.min_nodes; s.min_pct = sx.min_pct;
+    s.idx_in = words.d + 1; s.idx_out = words.d + 1; s.list = list.d; s.cnt = words.d;
+    s.soft_word = word.d; s.soft_seq = sx.seq;
+    k_evict_samp<true><<<1, 1024>>>(s);
+    EH_TRY(cudaGetLastError());
+  }
+  Mapped pick;
+  EH_TRY(pick.alloc(EV_PICK_K + 1));
+  p.pick_node = pick.d;
+  const size_t smem = (size_t)N * 8;
+  auto fn = sx.samp ? k_evict_pick<true, true> : k_evict_pick<false, true>;
+  auto fn_big = sx.samp ? k_evict_pick_big<true, true> : k_evict_pick_big<false, true>;
+  if (!sx.big && smem > 48 * 1024) EH_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int n_out = 0;
+  for (int seq = 1;; ++seq) {  // as the host control loop drains a ranking: until a batch comes back short
+    pick.h[EV_PICK_K] = ~seq;
+    if (sx.big) fn_big<<<1, 1024>>>(p, t.mode, seq);
+    else fn<<<1, 1024, smem>>>(p, t.mode, seq);
+    EH_TRY(cudaGetLastError());
+    EH_TRY(cudaDeviceSynchronize());
+    const volatile int32_t *h = pick.h;
+    if (h[EV_PICK_K] != seq) return EH_ECUDA;
+    int got = 0;
+    for (; got < EV_PICK_K && h[got] >= 0; ++got) {
+      if (n_out >= N) return EH_ECUDA;  // a node handed out twice
+      sx.order[n_out++] = h[got];
+    }
+    if (got < EV_PICK_K) break;
+  }
+  *sx.n_order = n_out;
+  EH_TRY(word.get(sx.word, 1));
+  return EH_OK;
+}
+
+static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx) {
   if (!a) return EH_EINVAL;
   const int N = a->N, R = a->R, RT = a->RT, J = a->J, Q = a->Q;
   if (N < 0 || R < 2 || R > VC_MAX_DIMS || RT < 0 || J < 0 || Q < 0 || a->pods_dim < -1 || a->pods_dim >= R) return EH_EINVAL;
@@ -195,6 +271,7 @@ extern "C" int eh_rank(const EhRankArgs *a) {
   t.qalloc_has = a->qalloc_has; t.qdes_has = a->qdes_has;
   if (a->quota_on)
     for (int d = 0; d < R; ++d) { t.qalloc[d] = a->qalloc[d]; t.qdes[d] = a->qdes[d]; }
+  if (sx) return soft_chain(a, *sx, p, t);
   if (N > 0) {  // the instance vcalloc.cu picks for R
     if (R <= 8) k_evict_rank<16, 8><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);
     else k_evict_rank<16, VC_MAX_DIMS><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);

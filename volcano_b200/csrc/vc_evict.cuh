@@ -66,6 +66,14 @@ struct EvictParams {
   const int32_t *samp_list, *samp_cnt;
   // apply command (mapped pinned memory): [0] node, [1] n_victims, [2..] victim running-task ids
   const int32_t *cmd;
+  // SOFT instances (preempt's normal reading with PreferNoSchedule taints under TaintToleration's batch score): the score
+  // is normalised by the largest intolerable-soft-taint count over predicateNodes, so it is final only after a reduction.
+  // k_evict_rank then stores the node's order part (the bits of a double) in `key`; soft_word holds
+  // (soft_seq << 8) | max — k_evict_rank's grid-wide max when soft_reduce, else k_evict_samp's over its list — and a word
+  // whose tag is not soft_seq was left by an earlier ranking and reads as 0. The pick finishes total_score per node.
+  unsigned long long *soft_word;
+  unsigned long long soft_seq;
+  int soft_klass, soft_reduce;
 };
 
 struct EvNodeView {
@@ -84,6 +92,20 @@ struct EvNodeView {
 __device__ __forceinline__ unsigned long long ev_score_key(double x) {  // monotone double -> u64
   unsigned long long u = (unsigned long long)__double_as_longlong(x);
   return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull);
+}
+
+// the soft-taint maximum of the ranking the pick reads (see EvictParams::soft_word)
+__device__ __forceinline__ int ev_max_soft(const EvictParams &p) {
+  const unsigned long long w = *p.soft_word;
+  return (w >> 8) == p.soft_seq ? (int)(w & 0xffull) : 0;
+}
+// the pick's order key of a node: SOFT adds TaintToleration's normalised score to the stored order part, in total_score's
+// operation order (0.0 + order, then + batch: the same double as a single call on the node)
+template <bool SOFT>
+__device__ __forceinline__ unsigned long long ev_pick_key(const EvictParams &p, int node, int max_soft) {
+  if (!SOFT) return p.key[node];
+  const int soft = (int)((p.cstat[(size_t)p.soft_klass * p.d.N + node] >> CS_SOFT_SHIFT) & 0xffu);
+  return ev_score_key(total_score(p.c, true, __longlong_as_double((long long)p.key[node]), soft, max_soft));
 }
 
 // the action's candidate filter on one task of node.Tasks
@@ -138,7 +160,9 @@ __device__ __forceinline__ bool ev_may_be_victim(const EvictParams &p, const Evi
 // that): the filters are chains of dependent loads (task -> job -> queue ...), so the walk is latency-bound and the lanes
 // overlap it; the requests of the possible victims are then summed per dimension with a shuffle tree inside the group.
 // The group's first lane scores the node when it is a candidate. RMAX bounds the resource dimensions (register budget).
-template <int LPN, int RMAX>
+// SOFT: the key is the order part only, and with soft_reduce every node passing the static predicate (candidate or not:
+// predicateNodes, scheduler_helper.go:76-136) enters the soft-taint maximum, one warp max and at most one atomic per warp.
+template <int LPN, int RMAX, bool SOFT = false>
 __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) {
   const size_t gid = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   const int n = (int)(gid / LPN);
@@ -169,6 +193,11 @@ __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) 
 #pragma unroll
     for (int d = 0; d < RMAX; ++d)
       if (d < R) freed[d] += __shfl_xor_sync(0xffffffffu, freed[d], o);
+  }
+  if (SOFT && p.soft_reduce) {
+    const unsigned sv = (stat_ok && gl == 0) ? ((cs >> CS_SOFT_SHIFT) & 0xffu) : 0u;
+    const unsigned long long w = (p.soft_seq << 8) | __reduce_max_sync(0xffffffffu, sv);
+    if ((threadIdx.x & 31) == 0 && *reinterpret_cast<volatile unsigned long long *>(p.soft_word) < w) atomicMax(p.soft_word, w);
   }
   if (!live || gl != 0) return;
   uint8_t cand = 0;
@@ -209,7 +238,8 @@ __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) 
         const EvNodeView nv{p, n};
         double order = 0.0;
         const bool has_order = node_order(p.c, R, K, t.rec, nv, cs, &order);
-        key = ev_score_key(total_score(p.c, has_order, has_order ? order : 0.0, 0, 0));
+        if (SOFT) key = (unsigned long long)__double_as_longlong(has_order ? order : 0.0);
+        else key = ev_score_key(total_score(p.c, has_order, has_order ? order : 0.0, 0, 0));
       }
     }
   }
@@ -224,8 +254,8 @@ __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) 
 // makes ONE thread rescan its nodes and ONE warp refold, the other 31 entries stay. Used when the keys do not fit in shared
 // memory (k_evict_pick below): repairs read the candidate flags and keys from global memory.
 // The last store of the launch is `seq` into pick_node[EV_PICK_K] (system scope): the host polls that word of the mapped
-// buffer instead of paying a stream synchronisation per hand-out.
-template <bool SAMP>
+// buffer instead of paying a stream synchronisation per hand-out. SOFT: the keys are finished here (ev_pick_key).
+template <bool SAMP, bool SOFT = false>
 __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
   __shared__ unsigned long long s_key[32];
   __shared__ int s_node[32];
@@ -234,6 +264,7 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
                                      // per iteration sits on the critical path of the block-wide barriers)
   const int N = SAMP ? *p.samp_cnt : p.d.N;  // SAMP: i walks the sampled list, node_of(i) is the node
   auto node_of = [&](int i) { return SAMP ? p.samp_list[i] : i; };
+  const int max_soft = SOFT ? ev_max_soft(p) : 0;
   if (threadIdx.x < EV_PICK_K) s_pick[threadIdx.x] = -1;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
   auto better_kn = [](unsigned long long ka, int na, unsigned long long kb, int nb) {
@@ -245,7 +276,7 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
     bk = 0ull; bn = -1;
     for (int n = threadIdx.x; n < N; n += blockDim.x) {
       if (n == skip || p.cand[node_of(n)] != 1) continue;
-      const unsigned long long k = mode == EV_MODE_RECLAIM ? 0ull : p.key[node_of(n)];
+      const unsigned long long k = mode == EV_MODE_RECLAIM ? 0ull : ev_pick_key<SOFT>(p, node_of(n), max_soft);
       if (bn < 0 || k > bk) { bk = k; bn = n; }  // ascending n per thread: the first of equal keys stays
     }
   };
@@ -302,9 +333,9 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
 // block barriers in all. Phase 1, every warp on its own 1/32 of the nodes: EV_PICK_K rounds of a warp arg-max (each lane
 // keeps the best of its ~N/1024 nodes in registers, the winner rescans its shared-memory entries) give the warp's first
 // EV_PICK_K candidates in order. Phase 2, one warp: a 32-way merge of those sorted lists. Same order as the sequential
-// tournament: key descending, node ascending.
+// tournament: key descending, node ascending. SOFT: the keys are finished while they are staged (ev_pick_key).
 extern __shared__ unsigned long long ev_pick_cache[];
-template <bool SAMP>
+template <bool SAMP, bool SOFT = false>
 __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, int seq) {
   __shared__ unsigned long long l_key[32][EV_PICK_K];
   __shared__ int l_node[32][EV_PICK_K];
@@ -312,8 +343,10 @@ __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, in
   const int N = SAMP ? *p.samp_cnt : p.d.N;  // SAMP: n walks the sampled list, node_of(n) is the node
   auto node_of = [&](int i) { return SAMP ? p.samp_list[i] : i; };
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int max_soft = SOFT ? ev_max_soft(p) : 0;
   for (int n = threadIdx.x; n < N; n += blockDim.x)  // key + 1 (never wraps: see ev_score_key), 0 = not a candidate
-    ev_pick_cache[n] = p.cand[node_of(n)] == 1 ? (mode == EV_MODE_RECLAIM ? 1ull : p.key[node_of(n)] + 1ull) : 0ull;
+    ev_pick_cache[n] = p.cand[node_of(n)] == 1 ? (mode == EV_MODE_RECLAIM ? 1ull : ev_pick_key<SOFT>(p, node_of(n), max_soft) + 1ull)
+                                               : 0ull;
   if (threadIdx.x < EV_PICK_K) s_pick[threadIdx.x] = -1;
   __syncwarp();  // a lane only ever reads the entries it wrote
   auto better_kn = [](unsigned long long ka, int na, unsigned long long kb, int nb) {
@@ -583,16 +616,22 @@ __global__ void __launch_bounds__(1024) k_evict_select(TopoSelect s) {
 // One block, as k_evict_select: every thread owns a contiguous chunk of nodes, a block scan gives the positions in the
 // scanned list and the ranks among the passing nodes; the rotated rank of a passing node counts from the first passing
 // node at or after `start`. idx_in may alias idx_out (read before the first barrier, written after the last).
+// SOFT: the largest soft-taint count over the kept nodes (TaintToleration's normalisation set under sampling) goes to
+// *soft_word as (soft_seq << 8) | max (EvictParams::soft_word).
 struct EvictSamp {
   const uint32_t *cstat;
   int klass, N, filtered;
   int pct, min_nodes, min_pct;  // vc_conf's percentage / minimum node count / minimum percentage to find
   const int32_t *idx_in;
   int32_t *idx_out, *list, *cnt;
+  unsigned long long *soft_word;
+  unsigned long long soft_seq;
 };
+template <bool SOFT = false>
 __global__ void __launch_bounds__(1024) k_evict_samp(EvictSamp s) {
   __shared__ int sp[1024], ss[1024];
   __shared__ int s_start, s_before, s_proc;
+  __shared__ unsigned s_soft;
   const int tid = threadIdx.x, nt = blockDim.x, N = s.N;
   const int chunk = (N + nt - 1) / nt;
   const int lo = min(N, tid * chunk), hi = min(N, lo + chunk);
@@ -604,7 +643,7 @@ __global__ void __launch_bounds__(1024) k_evict_samp(EvictSamp s) {
     cs += ok ? 1 : 0;
   }
   sp[tid] = cp; ss[tid] = cs;
-  if (tid == 0) { s_start = *s.idx_in; s_before = 0; s_proc = -1; }
+  if (tid == 0) { s_start = *s.idx_in; s_before = 0; s_proc = -1; s_soft = 0u; }
   __syncthreads();
   for (int o = 1; o < nt; o <<= 1) {  // inclusive scan
     const int a = tid >= o ? sp[tid - o] : 0, b = tid >= o ? ss[tid - o] : 0;
@@ -614,7 +653,10 @@ __global__ void __launch_bounds__(1024) k_evict_samp(EvictSamp s) {
   }
   const int P = sp[nt - 1], S = ss[nt - 1];
   if (P == 0) {
-    if (tid == 0) { *s.cnt = 0; *s.idx_out = s_start; }
+    if (tid == 0) {
+      *s.cnt = 0; *s.idx_out = s_start;
+      if (SOFT) *s.soft_word = s.soft_seq << 8;
+    }
     return;
   }
   const int start = s_start % P;
@@ -635,22 +677,28 @@ __global__ void __launch_bounds__(1024) k_evict_samp(EvictSamp s) {
   const int B = s_before;
   {
     int pi = sp[tid] - cp, si = ss[tid] - cs;
+    unsigned ms = 0u;
     for (int n = lo; n < hi; ++n) {
       const bool ok = pass(n);
       if (!ok && s.filtered) continue;
       if (ok) {
         const int rank = pi >= start ? si - B : (S - B) + si;
-        if (rank < M) s.list[rank] = n;
+        if (rank < M) {
+          s.list[rank] = n;
+          if (SOFT) ms = max(ms, (s.cstat[(size_t)s.klass * N + n] >> CS_SOFT_SHIFT) & 0xffu);
+        }
         if (rank == tf - 1) s_proc = (pi - start + P) % P + 1;  // the numNodesToFind-th node found: the scan stops there
         si += 1;
       }
       pi += 1;
     }
+    if (SOFT && ms) atomicMax(&s_soft, ms);
   }
   __syncthreads();
   if (tid == 0) {
     const int processed = s_proc >= 0 ? s_proc : P;
     *s.cnt = M;
     *s.idx_out = (int)(((long long)start + processed) % P);
+    if (SOFT) *s.soft_word = (s.soft_seq << 8) | s_soft;
   }
 }

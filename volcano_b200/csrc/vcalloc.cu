@@ -1834,8 +1834,8 @@ int ensure_evict_session(vc_snapshot *s) {
   if (s->dc.to_find > 0 && s->dc.enable_ecache && !s->all_pure)
     return fail(VC_EUNSUPPORTED, "preempt / reclaim under feasible-node sampling: enablePredicateErrorCache with a job whose "
                                  "named roles span several (class, request) groups (the role-keyed cache is not modelled)");
-  if (s->dc.soft_active || s->dc.nta_plugin || vch::has_plugin(s->conf, VC_PLUGIN_TDM))
-    return fail(VC_EUNSUPPORTED, "preempt / reclaim: PreferNoSchedule taints, network-topology-aware and tdm are outside the path");
+  if (s->dc.nta_plugin || vch::has_plugin(s->conf, VC_PLUGIN_TDM))
+    return fail(VC_EUNSUPPORTED, "preempt / reclaim: the network-topology-aware and tdm plugins are outside the path");
   for (uint8_t f : s->h_job_soft)
     if (f) return fail(VC_EUNSUPPORTED, "preempt / reclaim: jobs with a network topology (preempt.go:131-135)");
   if (s->es_built) return VC_OK;
@@ -1897,7 +1897,8 @@ int ensure_evict_session(vc_snapshot *s) {
                o_knz = take(K * B * 8), o_flags = take(B * 4), o_job = take(B * 4), o_ev = take(B), o_key = take(N * 8),
                o_cand = take(N), o_prio = take(B * 4), o_jready = take(std::max<size_t>(J, 1) * 4), o_qover = take(std::max<size_t>(Q, 1)),
                o_key2 = take(N * 8), o_cand2 = take(N),  // second ranking scratch: the preemptor ranked one ahead
-               o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4);  // k_evict_samp: lists, counts, indexes
+               o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4),  // k_evict_samp: lists, counts, indexes
+               o_soft = take(2 * 8);  // soft-taint maximum per ranking set (EvictParams::soft_word)
   if (off > s->d_ev_bytes) {
     if (s->d_ev) cudaFree(s->d_ev);
     s->d_ev = nullptr;
@@ -1905,7 +1906,7 @@ int ensure_evict_session(vc_snapshot *s) {
     s->d_ev_bytes = off;
   }
   if (!s->h_ev) CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&s->h_ev), (EV_CMD_OFF + 2 + EV_MAX_VICTIMS) * 4, cudaHostAllocMapped));
-  (void)o_key2; (void)o_cand2; (void)o_list; (void)o_list2; (void)o_samp;
+  (void)o_key2; (void)o_cand2; (void)o_list; (void)o_list2; (void)o_samp; (void)o_soft;
   unsigned char *base = reinterpret_cast<unsigned char *>(s->d_ev);
   CUDA_TRY(cudaMemsetAsync(base, 0, off, s->stream));
   if (s->rt.n > 0) {
@@ -1929,8 +1930,10 @@ int ensure_evict_session(vc_snapshot *s) {
 int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   if (!s || !out) return fail(VC_EINVAL, "null argument");
   if (!s->uploaded) return fail(VC_EINVAL, "vc_snapshot_upload must precede the action");
-  if (s->any_nominated)
-    return fail(VC_EUNSUPPORTED, "preempt / reclaim: a pending task carries a NominatedNodeName (taskEligibleToPreempt's rules are not modelled)");
+  // only preempt reads the nominated node (taskEligibleToPreempt, preempt.go:436-470); reclaim checks PreemptionPolicy
+  // alone (reclaim.go:140-143)
+  if (!reclaim && s->any_nominated)
+    return fail(VC_EUNSUPPORTED, "preempt: a pending task carries a NominatedNodeName (taskEligibleToPreempt's rules are not modelled)");
   if (s->hd_set)
     return fail(VC_EUNSUPPORTED, "preempt / reclaim with drf's enableHierarchy: the hdrf tree on evict events and hdrf's reclaimFn (drf.go:280-367) are not built");
   const double t0 = now_ms();
@@ -1948,7 +1951,8 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
                o_knz = take(K * B * 8), o_flags = take(B * 4), o_job = take(B * 4), o_ev = take(B), o_key = take(N * 8),
                o_cand = take(N), o_prio = take(B * 4), o_jready = take(std::max<size_t>(J, 1) * 4), o_qover = take(std::max<size_t>(Q, 1)),
                o_key2 = take(N * 8), o_cand2 = take(N),  // second ranking scratch: the preemptor ranked one ahead
-               o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4);  // k_evict_samp: lists, counts, indexes
+               o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4),  // k_evict_samp: lists, counts, indexes
+               o_soft = take(2 * 8);  // soft-taint maximum per ranking set (EvictParams::soft_word)
   unsigned char *base = reinterpret_cast<unsigned char *>(s->d_ev);
   EvictParams p;
   std::memset(&p, 0, sizeof p);
@@ -2057,13 +2061,22 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   int32_t *d_list[2] = {reinterpret_cast<int32_t *>(base + o_list), reinterpret_cast<int32_t *>(base + o_list2)};
   int idx_live = 2;
   if (samp) CUDA_TRY(cudaMemcpyAsync(d_samp + 4, &s->evict_idx, 4, cudaMemcpyHostToDevice, s->stream));
+  // PreferNoSchedule taints under TaintToleration's batch score change only the node order of preempt's normal reading
+  // (reclaim and the topology-aware reading walk nodes without scores): those rankings take the SOFT instances, each
+  // set's soft-taint maximum tagged with the sequence number of the ranking that wrote it (soft_seq[set])
+  const bool soft = !reclaim && !topo_on && s->dc.soft_active;
+  unsigned long long *d_soft = reinterpret_cast<unsigned long long *>(base + o_soft);
+  unsigned long long soft_seq[2] = {0, 0}, soft_next = 0;
+  int soft_klass[2] = {0, 0};
+  if (soft) CUDA_TRY(cudaMemsetAsync(d_soft, 0, 2 * 8, s->stream));  // words left by an earlier action read as no maximum
   auto launch_samp = [&](int set, int t) -> int {
     EvictSamp sa;
     sa.cstat = s->cstat; sa.klass = k.t_class[t]; sa.N = (int)N; sa.filtered = s->t_filtered[t];
     sa.pct = s->conf.percentage_nodes_to_find; sa.min_nodes = s->conf.min_nodes_to_find;
     sa.min_pct = s->conf.min_percentage_nodes_to_find;
     sa.idx_in = d_samp + 2 + idx_live; sa.idx_out = d_samp + 2 + set; sa.list = d_list[set]; sa.cnt = d_samp + set;
-    k_evict_samp<<<1, 1024, 0, s->stream>>>(sa);
+    sa.soft_word = d_soft + set; sa.soft_seq = soft_seq[set];
+    (soft ? k_evict_samp<true> : k_evict_samp<false>)<<<1, 1024, 0, s->stream>>>(sa);
     launches++;
     CUDA_TRY(cudaGetLastError());
     return VC_OK;
@@ -2089,9 +2102,12 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   int pick_buf[EV_PICK_K], pick_pos = EV_PICK_K, pick_n = 0;
   // the pick kernel stages the candidates' keys in shared memory when they fit (N * 8 bytes)
   size_t pick_smem = N * 8 <= 200 * 1024 ? N * 8 : 0;
+  void (*const pick_fn)(EvictParams, int, int) = samp ? (soft ? k_evict_pick<true, true> : k_evict_pick<true, false>)
+                                                      : (soft ? k_evict_pick<false, true> : k_evict_pick<false, false>);
+  void (*const pick_big_fn)(EvictParams, int, int) = samp ? (soft ? k_evict_pick_big<true, true> : k_evict_pick_big<true, false>)
+                                                          : (soft ? k_evict_pick_big<false, true> : k_evict_pick_big<false, false>);
   if (pick_smem > 48 * 1024)
-    CUDA_TRY(cudaFuncSetAttribute(samp ? k_evict_pick<true> : k_evict_pick<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)pick_smem));
+    CUDA_TRY(cudaFuncSetAttribute(pick_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pick_smem));
   double t_launch = 0.0, t_sync = 0.0;  // host time inside kernel launches / waiting for a hand-out (vc_stats.prof_cycles, us)
   // Two ranking scratch sets (candidate flags, keys, hand-out slots): while the host walks the candidates of one
   // preemptor the device already ranks the one the control loop will most likely try next (rk.hint). Most preemptors fail,
@@ -2108,21 +2124,29 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   auto with_set = [&](int k) {
     EvictParams q = p;
     q.key = sets[k].key; q.cand = sets[k].cand; q.pick_node = sets[k].d_pick; q.samp_list = d_list[k]; q.samp_cnt = d_samp + k;
+    q.soft_word = d_soft + k; q.soft_seq = soft_seq[k]; q.soft_klass = soft_klass[k]; q.soft_reduce = samp ? 0 : 1;
     return q;
   };
   auto launch_pick = [&](int k, int mode) -> int {
     sets[k].seq += 1;
-    if (pick_smem) (samp ? k_evict_pick<true> : k_evict_pick<false>)<<<1, 1024, pick_smem, s->stream>>>(with_set(k), mode, sets[k].seq);
-    else (samp ? k_evict_pick_big<true> : k_evict_pick_big<false>)<<<1, 1024, 0, s->stream>>>(with_set(k), mode, sets[k].seq);
+    if (pick_smem) pick_fn<<<1, 1024, pick_smem, s->stream>>>(with_set(k), mode, sets[k].seq);
+    else pick_big_fn<<<1, 1024, 0, s->stream>>>(with_set(k), mode, sets[k].seq);
     launches++;
     CUDA_TRY(cudaGetLastError());
     return VC_OK;
   };
   auto launch_rank_pick = [&](int k, int t, int mode) -> int {
     stage(t, mode);
+    if (soft) { soft_seq[k] = ++soft_next; soft_klass[k] = et.klass; }
     const double tl0 = now_ms();
-    if (R <= 8) k_evict_rank<16, 8><<<(unsigned)((N * 16 + 255) / 256), 256, 0, s->stream>>>(with_set(k), et);
-    else k_evict_rank<16, VC_MAX_DIMS><<<(unsigned)((N * 16 + 255) / 256), 256, 0, s->stream>>>(with_set(k), et);
+    const unsigned grid = (unsigned)((N * 16 + 255) / 256);
+    if (soft) {
+      if (R <= 8) k_evict_rank<16, 8, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
+      else k_evict_rank<16, VC_MAX_DIMS, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
+    } else {
+      if (R <= 8) k_evict_rank<16, 8><<<grid, 256, 0, s->stream>>>(with_set(k), et);
+      else k_evict_rank<16, VC_MAX_DIMS><<<grid, 256, 0, s->stream>>>(with_set(k), et);
+    }
     launches++;
     CUDA_TRY(cudaGetLastError());
     int rc2 = samp ? launch_samp(k, t) : VC_OK;
