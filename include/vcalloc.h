@@ -481,7 +481,9 @@ int vc_comm_prepare(vc_snapshot *s);
    A non-empty shard begins at a multiple of 64 (one mask word per shard); an empty one may begin anywhere. */
 int vc_snapshot_set_shard(vc_snapshot *s, int32_t node_begin, int32_t node_end);
 
-/* The allocate action on the uploaded snapshot: exact sequential greedy assignment. */
+/* The allocate action on the uploaded snapshot: exact sequential greedy assignment. VC_EUNSUPPORTED: feasible-node
+   sampling with min_nodes_to_find below 1 where numNodesToFind of the node list is 0 (the reference then finds no node
+   and advances lastProcessedNodeIndex by an amount that depends on its 16 workers). */
 int vc_allocate_run(vc_snapshot *s, vc_result **out);
 
 /* The backfill action (actions/backfill/backfill.go:58-116) on the session state vc_allocate_run left (or the
@@ -493,7 +495,8 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out);
    held (the tasks were dispatched to the binder) else VC_VISIT_KEEP (Allocated in the session only); tasks
    without a feasible node are listed in fit_errors. Feasible-node sampling continues from the lastProcessedNodeIndex
    the allocate run left (vc_stats.last_processed_node_index of this result carries it on). VC_EUNSUPPORTED: the
-   network-topology-aware plugin weighs a resource BestEffort pods request ("pods" in hypernode.binpack.resources). */
+   network-topology-aware plugin weighs a resource BestEffort pods request ("pods" in hypernode.binpack.resources), and
+   numNodesToFind 0 as for vc_allocate_run. */
 int vc_backfill_run(vc_snapshot *s, vc_result **out);
 
 /* The preempt action (actions/preempt/preempt.go:101-283, normalPreempt :333-434, or topologyAwarePreempt :475-1015 when

@@ -96,3 +96,53 @@ def test_pending_podgroups_without_the_enqueue_action(oracle_engine):
     o = OracleSession(snap)
     assert len(o.backfill_pick_order()) == 0
     o.close()
+
+
+def test_sampling_that_finds_no_node_on_the_oracle():
+    """min_nodes_to_find 0 and 10 nodes at 5 %: numNodesToFind is 0 (util/scheduler_helper.go:54-73), so every scan of
+    util.PredicateNodes finds nothing - allocate places no task and backfill lists every BestEffort task in fit_errors,
+    and the single-worker scan leaves lastProcessedNodeIndex where it was. The library refuses such a session."""
+    import dataclasses
+
+    from oracle import pyoracle
+    from volcano_b200.synth import CONFIGS
+    snap = make_snapshot(dataclasses.replace(CONFIGS["tiny_bf"], n_nodes=10, n_tasks=40, n_besteffort=20))
+    snap.conf.percentage_nodes_to_find, snap.conf.min_nodes_to_find, snap.conf.last_processed_node_index = 5, 0, 3
+    L = pyoracle.lib()
+    assert L.vco_num_feasible_nodes(10, 5, 0, snap.conf.min_percentage_nodes_to_find) == 0
+    o = OracleSession(snap)
+    dec, _, fe = o.allocate()
+    assert len(dec) == 0 and len(fe) > 0
+    order = o.backfill_pick_order()
+    dec, vis, fe = o.backfill()
+    assert len(order) > 0 and len(dec) == 0 and sorted(fe) == sorted(order)
+    assert L.vco_last_processed_node_index(o.h) == 3
+    o.close()
+    # one more node, or a minimum of 1, and the same session places pods again
+    snap.conf.min_nodes_to_find = 1
+    o = OracleSession(snap)
+    o.allocate()
+    assert len(o.backfill()[0]) > 0
+    o.close()
+
+
+def test_besteffort_jobs_knob():
+    """SynthConfig.besteffort_jobs puts every BestEffort pod into that many jobs; the default leaves the snapshot as it
+    was, and the regular part of the session never depends on it."""
+    import dataclasses
+
+    from volcano_b200.synth import CONFIGS
+    base = CONFIGS["small_bf"]
+    assert base.besteffort_jobs == 0
+    a = make_snapshot(base)
+    b = make_snapshot(dataclasses.replace(base, besteffort_jobs=0))
+    for k, v in a.__dict__.items():
+        if isinstance(v, np.ndarray):
+            assert np.array_equal(v, getattr(b, k)), k
+    for k, want in ((1, 1), (3, 3)):
+        c = make_snapshot(dataclasses.replace(base, besteffort_jobs=k))
+        assert len(np.unique(c.b_job)) == want and c.B == base.n_besteffort
+        assert np.all(np.diff(c.b_job) >= 0)
+        assert (c.j_pending_besteffort > 0).sum() == want and c.j_pending_besteffort.sum() == c.B
+        for name in ("t_resreq", "t_job", "t_klass", "n_idle", "n_label_bits", "c_selector", "j_queue"):
+            assert np.array_equal(getattr(a, name), getattr(c, name)), name

@@ -38,7 +38,10 @@ int fail(int code, const char *fmt, ...) {
 #define CUDA_TRY(x)                                                                     \
   do {                                                                                  \
     cudaError_t e_ = (x);                                                               \
-    if (e_ != cudaSuccess) return fail(VC_ECUDA, "%s: %s", #x, cudaGetErrorString(e_)); \
+    if (e_ != cudaSuccess) {                                                            \
+      cudaGetLastError(); /* a non-sticky error must not fail the next call's check */  \
+      return fail(VC_ECUDA, "%s: %s", #x, cudaGetErrorString(e_));                      \
+    }                                                                                   \
   } while (0)
 
 // mailbox: two parities x up to 2048 CTA slots (several ranks) of MBOX_STRIDE uint4; a second region of the same size serves
@@ -374,6 +377,15 @@ int build_devconf(vc_snapshot *s, const vc_nodes *nd) {
     if (nd->taint_soft && nd->taint_soft[i]) soft = 1;
   d.soft_active = d.taint_batch && soft;
   return VC_OK;
+}
+
+// numNodesToFind == 0 (min-nodes-to-find below 1 and a percentage that rounds down to no node): util.PredicateNodes
+// finds no node, and how far its 16 workers move lastProcessedNodeIndex before the first feasible node cancels them is
+// not determined. d.to_find cannot tell this case from "no sampling", so allocate and backfill refuse it.
+bool samples_no_node(const vc_snapshot *s) {
+  const int32_t N = s->dims.n_nodes;
+  return N > 0 && vch::num_feasible_nodes_to_find(N, s->conf.percentage_nodes_to_find, s->conf.min_nodes_to_find,
+                                                  s->conf.min_percentage_nodes_to_find) <= 0;
 }
 
 // smallest launch geometry that keeps one node per thread when possible
@@ -1475,6 +1487,8 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   if (s->dd.node_begin != 0 || s->dd.node_end != (int)N)
     return fail(VC_EUNSUPPORTED, "the commit engine takes the full node axis (vc_comm_create cuts it over the ranks itself)");
   if (s->world > 1 && !s->comm_attached) return fail(VC_EINVAL, "vc_comm_attach must precede vc_allocate_run");
+  if (T > 0 && samples_no_node(s))
+    return fail(VC_EUNSUPPORTED, "allocate under feasible-node sampling: min-nodes-to-find below 1 and numNodesToFind 0");
   const int G = s->n_cta;
   // replicas, mailbox, outputs
   const size_t i32_stride = ((5 * J + 4 * NR + 5 * Q + 3 * (size_t)s->max_job_tasks) + 63) & ~(size_t)63;
@@ -2495,6 +2509,10 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
   vc_result *r = new vc_result();
   r->stats.upload_ms = s->upload_ms;
   if (B > 0 && s->dc.to_find > 0 && s->npc > 4 * s->block) { delete r; return fail(VC_EUNSUPPORTED, "feasible-node sampling: more than 4 x blockDim nodes per CTA"); }
+  if (B > 0 && samples_no_node(s)) {
+    delete r;
+    return fail(VC_EUNSUPPORTED, "backfill under feasible-node sampling: min-nodes-to-find below 1 and numNodesToFind 0");
+  }
   if (B > 0 && s->dc.nta_on) {
     // hypernode binpacking of a BestEffort pod: every term is skipped unless a weighted resource is requested
     // (network_topology_aware.go:507-520), i.e. unless "pods" is listed in hypernode.binpack.resources
@@ -2587,7 +2605,11 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
   std::memcpy(stage.data() + o_klass, bf.klass.data(), B * 4);
   std::memcpy(stage.data() + o_group, group.data(), B * 4);
   if (n) std::memcpy(stage.data() + o_order, order.data(), n * 4);
-  auto bail = [&](cudaError_t e, const char *what) { delete r; return fail(VC_ECUDA, "%s: %s", what, cudaGetErrorString(e)); };
+  auto bail = [&](cudaError_t e, const char *what) {
+    delete r;
+    cudaGetLastError();  // a non-sticky error must not fail the next call's check
+    return fail(VC_ECUDA, "%s: %s", what, cudaGetErrorString(e));
+  };
   cudaError_t e = cudaMemcpyAsync(s->d_bf, stage.data(), in_bytes, cudaMemcpyHostToDevice, s->stream);
   if (e != cudaSuccess) return bail(e, "backfill H2D");
   if (!s->alloc_ran) {  // no allocate action in this cycle: start from the opening node state

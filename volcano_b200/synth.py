@@ -40,6 +40,8 @@ class SynthConfig:
     topology_scatter: float = 0.0     # fraction of nodes assigned to a random leaf / left outside the tree (tests)
     soft_topology_frac: float = 0.0   # fraction of jobs whose PodGroup carries a soft-mode network topology
     n_besteffort: int = 0             # extra BestEffort pending pods spread over the jobs (the backfill action's tasks)
+    besteffort_jobs: int = 0          # > 0: the BestEffort pods go into that many random jobs only (long same-group runs
+                                      # in backfill's pick order); 0: spread over all jobs
     hetero: int = 0                   # > 0: every task draws its own request from `hetero` distinct cpu / memory sizes
                                       # (heterogeneous pods: the (class, request) groups of the dense pass approach T)
     hdrf: Optional[tuple] = None      # (departments, teams): drf's enableHierarchy over a root -> department -> team tree
@@ -360,7 +362,11 @@ def _make_besteffort(s: Snapshot, cfg: SynthConfig, rng, job_class) -> None:
     """BestEffort pending pods (Resreq = pods:1 only; upstream non-zero defaults 100m / 200Mi for the scorers) attached to
     random jobs: they count in PendingBestEffortTaskNum / the role's occupancy during allocate and are placed by backfill."""
     B, J = cfg.n_besteffort, s.J
-    bj = np.sort(rng.integers(0, J, B)).astype(np.int32)
+    if cfg.besteffort_jobs > 0:
+        hosts = rng.choice(J, size=min(cfg.besteffort_jobs, J), replace=False)
+        bj = np.sort(hosts[rng.integers(0, len(hosts), B)]).astype(np.int32)
+    else:
+        bj = np.sort(rng.integers(0, J, B)).astype(np.int32)
     s.b_job[:] = bj
     s.b_klass[:] = job_class[bj]
     s.b_role[:] = s.j_role_off[bj]  # first role row of the job
