@@ -52,7 +52,7 @@
 extern "C" {
 #endif
 
-#define VC_ABI_VERSION 5
+#define VC_ABI_VERSION 6
 #define VC_MAX_DIMS 16   /* R  */
 #define VC_MAX_KDIMS 4   /* dims seen by the upstream kube-scheduler scorers (cpu, memory, nvidia.com/gpu, ...) */
 #define VC_MAX_WORDS 4   /* 64-bit words per label / taint bitset */
@@ -377,6 +377,9 @@ typedef struct vc_stats {
                              gates, 2 node sweep, 3 mailbox exchange, 4 apply + bookkeeping */
   int32_t last_processed_node_index; /* util.lastProcessedNodeIndex after the cycle (to carry into the next one) */
   int32_t commit_kernel; /* which instance of the commit kernel served the cycle: VC_KERNEL_* (diagnostic) */
+  int32_t group_reentry[4]; /* VC_PROF instance of the incremental kernel: 0 group switches served by a full sweep, 1 those
+                               served from the per-group verdict table (control program of CTA 0); 2 rows re-evaluated on
+                               re-entry, 3 re-entries of a CTA past its changed-row threshold (both summed over CTAs) */
 } vc_stats;
 #define VC_KERNEL_GENERAL 0      /* k_commit: full sweep + all-gather per placement */
 #define VC_KERNEL_INCREMENTAL 1  /* k_commit_fast: verdict cache, single-record publications, run-length batches */

@@ -32,6 +32,7 @@ out = {"cfg": cfg, "ctas": os.environ.get("VC_COMMIT_CTAS"), "threads": os.envir
        "placed": len(r.decisions), "us_per_step": 1e3 * st["commit_ms"] / max(1, st["n_steps"]),
        "cycles_per_step": tot / max(1, st["n_steps"]),
        "phases": {n: round(p / tot, 3) for n, p in zip(names, prof)},
-       "pods_per_s": len(r.decisions) / (st["commit_ms"] * 1e-3), "full_sweeps": prof[6], "incremental": prof[7], "owner_changes": prof[5]}
+       "pods_per_s": len(r.decisions) / (st["commit_ms"] * 1e-3), "full_sweeps": prof[6], "incremental": prof[7], "owner_changes": prof[5],
+       "group_reentry": st["group_reentry"]}
 print(json.dumps(out))
 e.close()

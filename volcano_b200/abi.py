@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 
-VC_ABI_VERSION = 5
+VC_ABI_VERSION = 6
 VC_MAX_DIMS = 16
 VC_MAX_KDIMS = 4
 VC_MAX_WORDS = 4
@@ -236,7 +236,8 @@ class vc_stats(C.Structure):
     _fields_ = [("upload_ms", C.c_double), ("commit_ms", C.c_double), ("download_ms", C.c_double),
                 ("total_ms", C.c_double), ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64),
                 ("kernel_launches", C.c_int32), ("n_steps", C.c_int32), ("prof_cycles", C.c_int64 * 8),
-                ("last_processed_node_index", C.c_int32), ("commit_kernel", C.c_int32)]
+                ("last_processed_node_index", C.c_int32), ("commit_kernel", C.c_int32),
+                ("group_reentry", C.c_int32 * 4)]
 
 
 # every symbol include/vcalloc.h declares: name -> (restype, argtypes)

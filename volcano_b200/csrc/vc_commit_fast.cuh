@@ -103,7 +103,15 @@ struct FastParams {  // extra kernel arguments of the fast kernel
   int run_max;             // 1: one placement per publication; RUN_MAX: run-length batches (rows integer-valued)
   uint4 *score_log;        // [T] per placement attempt inside a run: (score bits lo, hi, attempt index + 1, 0), written by the
                            // owner CTA as one 16-byte store and polled by CTA 0 - the tag makes a fence before the record unnecessary
+  // per-group verdict table (nullptr: the session is over the table's memory budget and re-enters a group with a full
+  // sweep): category and score of every (group, node of this rank) as they were when the group's cache was last current
+  uint8_t *vt_cat;         // [n_groups][gridDim.x * npc]
+  double *vt_score;        // [n_groups][gridDim.x * npc]
+  int32_t *vt_gstamp;      // [gridDim.x][n_groups] per-CTA replica of the group stamps (-1: no saved verdicts this cycle)
 };
+// Above this many changed rows in a CTA, a re-entry evaluates them one per thread (one pass, like a full sweep) instead of
+// in warp-cooperative rounds of 2 rows per warp
+#define VT_DIRTY_MAX 32
 
 struct FastSmem {
   double *alloc, *idle, *used, *kalloc, *kreq, *knz;
@@ -115,6 +123,8 @@ struct FastSmem {
   double *sl_score;
   int32_t *sl_node, *sl_cnt, *sl_cat;
   int32_t *sl_feas;  // SAMP: feasible nodes (category 0 or 1) of every CTA for the cached group
+  int32_t *mstamp;   // value of the control program's verdict clock at the last change of each row
+  int32_t *dlist;    // rows a re-entry re-evaluates
   int cap;
 };
 struct FastNodeView {
@@ -360,6 +370,12 @@ struct CtlFast {  // shared-memory state of the fast kernel next to Ctl
   // CMD_RUN: placements the control program allows on node ev_i in a row (run_L), attempt index of the first one,
   // result (run_m placements made), runner-up computed by warp 2
   int run_L, run_att0, run_m;
+  // full sweep / re-entry command: group whose cached verdicts are saved to the table first (-1: none), re-entry (1) or
+  // full sweep (0), verdicts taken from the table (else the CTA's cache already holds the group), stamp of the saved
+  // verdicts, rows found changed; rollback command: stamp of the rows it changes
+  int vt_wb, vt_reenter, vt_load, vt_stamp, vt_nd;
+  int vt_clock, vt_held, vt_held_stamp;  // control state of the verdict table (see the control program)
+  int vt_n[2];  // VC_PROF: group switches served by a full sweep / from saved verdicts
   double ru_score, rl_score;
   int ru_node, rl_node, rl_cnt;
   int ru_cat, rl_cat, rl_cnt0, rl_cnt1;
@@ -421,6 +437,8 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
   fs.nerr_stamp = reinterpret_cast<int32_t *>(sp); sp += (size_t)cap * 4;
   fs.c_cat = reinterpret_cast<int32_t *>(sp); sp += (size_t)cap * 4;
   fs.c_cs = reinterpret_cast<uint32_t *>(sp); sp += (size_t)cap * 4;
+  fs.mstamp = reinterpret_cast<int32_t *>(sp); sp += (size_t)cap * 4;
+  fs.dlist = reinterpret_cast<int32_t *>(sp); sp += (size_t)cap * 4;
   fs.sl_node = reinterpret_cast<int32_t *>(sp); sp += (size_t)G * 4;
   fs.sl_cnt = reinterpret_cast<int32_t *>(sp); sp += (size_t)G * 4;
   fs.sl_cat = reinterpret_cast<int32_t *>(sp); sp += (size_t)G * 4;
@@ -449,8 +467,18 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
     fs.c_cat[i] = 2;
     fs.c_score[i] = 0.0;
     fs.c_cs[i] = 0u;
+    fs.mstamp[i] = 0;
   }
   for (int s = tid; s < G; s += blockDim.x) { fs.sl_score[s] = 0.0; fs.sl_node[s] = -1; fs.sl_cnt[s] = 0; fs.sl_cat[s] = 0; fs.sl_feas[s] = 0; }
+  // Per-group verdict table (not the SOFT instance: its cached scores carry normalisation constants that move). The table
+  // itself is not cleared between cycles: a group's entries count only once its stamp was set in this launch.
+  // (entry of row i of group g: g * gridDim.x * npc + blockIdx.x * npc + i; recomputed where used, like VT, to keep
+  //  them out of the registers of the control warp)
+#define VT (!SOFT && fp.vt_cat != nullptr)
+#define VT_AT(g, i) ((size_t)(g) * gridDim.x * p.npc + (size_t)blockIdx.x * p.npc + (i))
+#define VT_GSTAMP(g) fp.vt_gstamp[(size_t)blockIdx.x * p.n_groups + (g)]
+  if (VT)
+    for (int g = tid; g < p.n_groups; g += blockDim.x) VT_GSTAMP(g) = -1;
 
   // ---- per-CTA replica of the mutable control state, packed records ----
   unsigned char *rb = reinterpret_cast<unsigned char *>(p.rep_f64 + (size_t)lcta * p.rep_f64_stride);
@@ -493,8 +521,52 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
     F.cta_best_node = -1; F.cta_cnt = 0; F.g_best_node = -1; F.g_cnt = 0; F.cta_best_score = F.g_best_score = 0.0;
     F.cta_best_cat = 0; F.cta_cnt1 = 0; F.ev_kind = 0; F.ev_cat = 0; F.ev_flag = 0; F.g_soft[0] = F.g_soft[1] = 0;
     F.spec_i[0] = F.spec_i[1] = -1;
+    F.vt_wb = -1; F.vt_reenter = 0; F.vt_load = 0; F.vt_stamp = -1; F.vt_nd = 0;
+    F.vt_clock = 0; F.vt_held = -1; F.vt_held_stamp = -1; F.vt_n[0] = F.vt_n[1] = 0;
   }
   __syncthreads();
+
+  // per-warp result of a sweep: best (score, node, category) and, FUT, how many of the warp's nodes sit in category 0 / 1
+  auto post_warp = [&](Best &b, int n0, int n1) {
+    best_warp_reduce<FUT>(b);
+    if (FUT) {
+      n0 = (int)__reduce_add_sync(0xffffffffu, (unsigned)n0);
+      n1 = (int)__reduce_add_sync(0xffffffffu, (unsigned)n1);
+    }
+    if (lane == 0) {
+      S.w_score[0][warp] = b.score; S.w_node[0][warp] = b.node; S.w_cnt[0][warp] = FUT ? n0 : b.cnt;
+      if (FUT) { S.w_cnt[1][warp] = n1; S.w_node[1][warp] = b.cat; }
+    }
+  };
+  // verdict of row i for the staged group record, one thread (the same operations as eval_dirty, one after the other)
+  auto eval_full = [&](int i, uint32_t cs, double *sc) -> int {
+    const TaskRec &trec = S.trec;
+    FastNodeView nv{fs, i};
+    const bool pod_cap = c.pred_predicates && fs.max_tasks[i] <= fs.pod_count[i];
+    int cat = eval_pair_fast<SOFT>(c, R, K, trec, nv, cs, pod_cap, sc);
+    if (FUT) {
+      // alloc.predicate: InitResreq <= FutureIdle (allocate.go:816-824); the idle gradient is the subset that fits
+      // Idle as well (:722-733). eval_pair_fast answered 0 exactly when the static part, the pod count AND Idle pass.
+      bool fit_future = (cs & CS_STATIC_OK) != 0 && !pod_cap;
+      for (int d = 0; d < R; ++d) {
+        if (d >= 2 && !(trec.has & (1u << d))) continue;
+        const double fut = (fs.idle[d * cap + i] + fs.rel[d * cap + i]) - fs.pip[d * cap + i];
+        if (!le_eps(trec.req[d], fut)) fit_future = false;
+      }
+      cat = !fit_future ? 2 : (cat == 0 ? 0 : 1);
+    }
+    return cat;
+  };
+  // before a sweep or a re-entry overwrites the verdict cache: save the verdicts of the group it holds (F.vt_wb) to the
+  // table (each thread its own rows, which it overwrites after this)
+  auto vt_save = [&]() {
+    const int wb = F.vt_wb;
+    if (wb < 0) return;
+    for (int i = tid; i < nmine; i += blockDim.x) {
+      fp.vt_cat[VT_AT(wb, i)] = (uint8_t)fs.c_cat[i];
+      fp.vt_score[VT_AT(wb, i)] = fs.c_score[i];
+    }
+  };
 
   // full evaluation of this thread's nodes for the staged group record (command CMD_SWEEP)
   auto sweep_part = [&]() {
@@ -505,6 +577,7 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
     const int vid = S.visit_id;
     Best b{0.0, -1, 0, 0};
     int n0 = 0, n1 = 0;
+    if (!SOFT) vt_save();  // (F.vt_wb stays -1 without a table)
     if (SOFT && S.cmd == CMD_SWEEP2) {
       // second phase: TaintToleration's normalised score joins the cached NodeOrderFn sums (scheduler_helper.go:117-129)
       const int gs0 = F.g_soft[0], gs1 = F.g_soft[1];
@@ -517,38 +590,17 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
         best_fold(b, sc, nbase + i, 1, cat);
         if (FUT) { n0 += cat == 0; n1 += cat == 1; }
       }
-      best_warp_reduce<FUT>(b);
-      if (FUT) {
-        n0 = (int)__reduce_add_sync(0xffffffffu, (unsigned)n0);
-        n1 = (int)__reduce_add_sync(0xffffffffu, (unsigned)n1);
-      }
-      if (lane == 0) {
-        S.w_score[0][warp] = b.score; S.w_node[0][warp] = b.node; S.w_cnt[0][warp] = FUT ? n0 : b.cnt;
-        if (FUT) { S.w_cnt[1][warp] = n1; S.w_node[1][warp] = b.cat; }
-      }
+      post_warp(b, n0, n1);
       return;
     }
     int ms0 = 0, ms1 = 0;  // SOFT, first phase: largest soft-taint count among this thread's candidates per category
     for (int i = tid; i < nmine; i += blockDim.x) {
-      FastNodeView nv{fs, i};
       const uint32_t cs = __ldg(cs_row + i);
       if (use_cache && fs.nerr_stamp[i] != vid) { fs.nerr[i] = 0ull; fs.nerr_stamp[i] = vid; }
       int cat = 2;
       double sc = 0.0;
       if (!(use_cache && ((fs.nerr[i] >> rl) & 1ull))) {
-        const bool pod_cap = c.pred_predicates && fs.max_tasks[i] <= fs.pod_count[i];
-        cat = eval_pair_fast<SOFT>(c, R, K, trec, nv, cs, pod_cap, &sc);
-        if (FUT) {
-          // alloc.predicate: InitResreq <= FutureIdle (allocate.go:816-824); the idle gradient is the subset that fits
-          // Idle as well (:722-733). eval_pair_fast answered 0 exactly when the static part, the pod count AND Idle pass.
-          bool fit_future = (cs & CS_STATIC_OK) != 0 && !pod_cap;
-          for (int d = 0; d < R; ++d) {
-            if (d >= 2 && !(trec.has & (1u << d))) continue;
-            const double fut = (fs.idle[d * cap + i] + fs.rel[d * cap + i]) - fs.pip[d * cap + i];
-            if (!le_eps(trec.req[d], fut)) fit_future = false;
-          }
-          cat = !fit_future ? 2 : (cat == 0 ? 0 : 1);
-        }
+        cat = eval_full(i, cs, &sc);
         if (cat == 2 && use_cache) fs.nerr[i] |= (1ull << rl);
       }
       fs.c_cat[i] = cat;
@@ -569,24 +621,18 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
       if (lane == 0) { S.w_soft[0][warp] = ms0; S.w_soft[1][warp] = ms1; }
       return;
     }
-    best_warp_reduce<FUT>(b);
-    if (FUT) {
-      n0 = (int)__reduce_add_sync(0xffffffffu, (unsigned)n0);
-      n1 = (int)__reduce_add_sync(0xffffffffu, (unsigned)n1);
-    }
-    if (lane == 0) {
-      S.w_score[0][warp] = b.score; S.w_node[0][warp] = b.node; S.w_cnt[0][warp] = FUT ? n0 : b.cnt;
-      if (FUT) { S.w_cnt[1][warp] = n1; S.w_node[1][warp] = b.cat; }
-    }
+    post_warp(b, n0, n1);
   };
   // stmt.Discard() for this thread's nodes (command CMD_DISCARD), statement.go:357-381
   auto discard_part = [&]() {
     const int n_ops = S.n_ops;
+    const int vclk = F.vt_clock;
     for (int k = n_ops - 1; k >= 0; --k) {
       const int ot = ops[k * 3 + 0], on = ops[k * 3 + 1];
       const bool was_pipe = FUT && ops[k * 3 + 2] == VC_OP_PIPELINE;
       if (on >= nbase && on < nbase + nmine && ((on - nbase) % blockDim.x) == tid) {
         const int i = on - nbase;
+        fs.mstamp[i] = vclk;
         for (int d = 0; d < R; ++d) {
           double rq = p.req[(size_t)d * T + ot];
           if (was_pipe) { fs.pip[d * cap + i] -= rq; continue; }
@@ -787,6 +833,55 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
     int wv = (role == ROLE_BP && on_task) ? w_d : 0;
     for (int o = 4; o; o >>= 1) wv += __shfl_xor_sync(0xffffffffu, wv, o);  // lane 0: sum over lanes 0-7 (every 8-lane group sums its own)
     wsum_g = __shfl_sync(0xffffffffu, wv, 0);
+  };
+  // Re-entry of the staged group (command CMD_SWEEP with F.vt_reenter, every warp, operands staged): rows unchanged since
+  // the group's verdicts were saved (stamp <= F.vt_stamp) take them from the table (or keep them, when this CTA's cache
+  // still holds the group); the changed ones are re-evaluated - two per worker warp and round, or one per thread past
+  // VT_DIRTY_MAX - and the CTA's rows are folded as a sweep folds them. (The control warp takes no round: the
+  // warp-cooperative evaluator in its code would cost it registers it does not have to spare.)
+  int vt_rows = 0, vt_fallback = 0;  // VC_PROF: rows re-evaluated on re-entry, re-entries past VT_DIRTY_MAX (thread 0)
+  auto reenter_part = [&](bool rounds) {
+    const int g = F.cur_group, st = F.vt_stamp;
+    const bool load = F.vt_load != 0;
+    const uint32_t *cs_row = p.cstat + (size_t)S.trec.klass * N + nbase;
+    vt_save();
+    for (int i = tid; i < nmine; i += blockDim.x) {
+      fs.c_cs[i] = __ldg(cs_row + i);
+      if (fs.mstamp[i] > st) {
+        fs.dlist[atomicAdd(&F.vt_nd, 1)] = i;
+      } else if (load) {
+        fs.c_cat[i] = fp.vt_cat[VT_AT(g, i)];
+        fs.c_score[i] = fp.vt_score[VT_AT(g, i)];
+      }
+    }
+    __syncthreads();
+    const int nd = F.vt_nd;
+    if (nd > VT_DIRTY_MAX) {
+      for (int k = tid; k < nd; k += blockDim.x) {
+        const int i = fs.dlist[k];
+        double sc = 0.0;
+        const int cat = eval_full(i, fs.c_cs[i], &sc);
+        fs.c_cat[i] = cat; fs.c_score[i] = sc;
+      }
+    } else if (rounds) {
+      for (int pr = warp - 1; 2 * pr < nd; pr += nwarps - 1) {
+        const bool two = 2 * pr + 1 < nd;
+        const int i0 = fs.dlist[2 * pr], i1 = two ? fs.dlist[2 * pr + 1] : i0;
+        double sc = 0.0;
+        const int cat = eval_dirty(i0, i1, 0, 0, fs.c_cs[half ? i1 : i0], &sc);
+        if (hl == 0 && (half == 0 || two)) { fs.c_cat[half ? i1 : i0] = cat; fs.c_score[half ? i1 : i0] = sc; }
+      }
+    }
+    if (PROF && tid == 0) { vt_rows += nd; vt_fallback += nd > VT_DIRTY_MAX ? 1 : 0; }
+    __syncthreads();
+    Best b{0.0, -1, 0, 0};
+    int n0 = 0, n1 = 0;
+    for (int i = tid; i < nmine; i += blockDim.x) {
+      const int cat = fs.c_cat[i];
+      if (cat == 0 || (FUT && cat == 1)) best_fold(b, fs.c_score[i], nbase + i, 1, cat);
+      if (FUT) { n0 += cat == 0; n1 += cat == 1; }
+    }
+    post_warp(b, n0, n1);
   };
   // CMD_EVAL (warp 1): re-evaluate node F.ev_i for the cached group, maintain this CTA's best incrementally
   // (rescan only when the holder got worse) and publish the CTA's new best in the ring.
@@ -996,7 +1091,11 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
         if (PROF && warp == 2 && lane == 0) atomicAdd(&p.counters[12], (int)(ev_acc_spec >> 10));
         break;
       }
-      if (cmd == CMD_SWEEP || cmd == CMD_SWEEP2) sweep_part();
+      if (!SOFT && cmd == CMD_SWEEP && F.vt_reenter) {
+        if (F.cur_group != my_group) { stage_ops(); my_group = F.cur_group; }
+        reenter_part(true);
+      }
+      else if (cmd == CMD_SWEEP || cmd == CMD_SWEEP2) sweep_part();
       else if (cmd == CMD_DISCARD) discard_part();
       else if (cmd == CMD_RUN) {  // all worker warps, joined on named barrier 2; warp 1 signals warp 0 on barrier 1
         if (F.cur_group != my_group) { stage_ops(); my_group = F.cur_group; }
@@ -1060,6 +1159,22 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
     unsigned pub_pc = 0;
     int n_att = 0;   // placement attempts so far (index into the score log; every task is attempted at most once)
     int pub_m = 1;   // placements covered by the publication resolve() consumed last
+    // Per-group verdict table. F.vt_clock: a clock that advances each time a group's cache stops being current (the
+    // group's stamp takes its value first); every change of a row stamps the row with it, so the rows a group has to
+    // re-evaluate on re-entry are exactly those with a larger stamp. F.vt_held: the group whose verdicts the CTA's cache
+    // holds, exact for every row stamped at most F.vt_held_stamp (or current, when it is cache_group). (Shared memory,
+    // written by lane 0: the control warp has no registers to spare for them.)
+    auto vt_stop = [&]() {
+      if (!VT || cache_group < 0) return;
+      __syncwarp();
+      if (lane == 0) {
+        const int clk = F.vt_clock;
+        VT_GSTAMP(cache_group) = clk;
+        F.vt_held_stamp = clk;
+        F.vt_clock = clk + 1;
+      }
+      __syncwarp();
+    };
 
     // Visit state that survives from one visit to the next: a re-pushed job is usually popped again right away
     // (one task per visit once it is Ready, allocate.go:676), and a session often has few queues — so the queue
@@ -1371,10 +1486,26 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
 
       // full sweep of this CTA's nodes for the staged group (every warp), reduced to the CTA's best and, for the FUT
       // instance, its node counts per category
-      auto sweep_local = [&](int rl, bool use_cache, Best &mine, int &c0, int &c1) {
+      // (a pure job's group with verdicts saved this cycle re-enters from them: see reenter_part)
+      auto sweep_local = [&](int grp, int rl, bool use_cache, Best &mine, int &c0, int &c1) {
+          bool reenter = false;
+          if (VT) {
+            vt_stop();
+            int st = -1;
+            if (lane == 0) {
+              const int held = F.vt_held;
+              if (pure) st = held == grp ? F.vt_held_stamp : VT_GSTAMP(grp);
+              F.vt_wb = (held >= 0 && !(st >= 0 && held == grp)) ? held : -1;
+              F.vt_reenter = st >= 0 ? 1 : 0; F.vt_load = held != grp ? 1 : 0; F.vt_stamp = st; F.vt_nd = 0;
+              F.vt_held = pure ? grp : -1;
+            }
+            reenter = __shfl_sync(0xffffffffu, st, 0) >= 0;
+          }
+          if (PROF && lane == 0) F.vt_n[reenter ? 1 : 0] += 1;
           if (lane == 0) { S.cmd = CMD_SWEEP; S.sweep_rl = rl; S.sweep_use_cache = use_cache ? 1 : 0; S.visit_id = visit_id; }
           __syncthreads();  // B1
-          sweep_part();
+          if (!SOFT && reenter) reenter_part(false);
+          else sweep_part();
           __syncthreads();  // B2
           if (SOFT) {
             // first phase done (verdicts, NodeOrderFn sums, per-warp soft-taint maxima): all-gather the maxima, then the
@@ -1491,7 +1622,7 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
             resolve();
             Best mine{0.0, -1, 0, 0};
             int c0 = 0, c1 = 0;
-            sweep_local(rl, use_cache, mine, c0, c1);
+            sweep_local(grp, rl, use_cache, mine, c0, c1);
             const int feas = FUT ? c0 + c1 : mine.cnt;
             if (lane == 0) {
               F.cta_best_score = mine.score; F.cta_best_node = mine.node;
@@ -1739,7 +1870,7 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
           // -------- full sweep --------
           Best mine{0.0, -1, 0, 0};
           int c0 = 0, c1 = 0;
-          sweep_local(rl, use_cache, mine, c0, c1);
+          sweep_local(grp, rl, use_cache, mine, c0, c1);
           exchange_all_fast(p, mine, ag, fs);
           Best g = fold_slots<FUT>(fs, G, &g_best_owner);
           ag += 1; since_sync = 0; n_full += 1;
@@ -1794,6 +1925,8 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
         // ---- Statement.Allocate / Pipeline: node.AddTask on the owner CTA (api/node_info.go:435-484) ----
         if (best >= nbase && best < nbase + nmine) {
           const int i = best - nbase;
+          // (the further placements of a run on this row happen before vclk moves: this stamp covers them)
+          if (!SOFT && lane == 0) fs.mstamp[i] = F.vt_clock;
           if (lane < R) {
             if (pipe) {
               fs.pip[lane * cap + i] += req_l;
@@ -1970,6 +2103,7 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
       }
       if (!stmt && n_ops > 0) {
         resolve();  // the evaluator must be idle and the slot table current before nodes are rolled back
+        vt_stop();  // (the cache keeps the group's verdicts; a re-entry re-evaluates the rows rolled back)
         if (lane == 0) { S.cmd = CMD_DISCARD; S.n_ops = n_ops; }
         __syncthreads();  // B1
         discard_part();
@@ -2090,6 +2224,8 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
       atomicAdd((unsigned long long *)&p.prof[13], (unsigned long long)acc_ab);
       atomicAdd((unsigned long long *)&p.prof[14], (unsigned long long)acc_bc);
       atomicAdd((unsigned long long *)&p.prof[15], (unsigned long long)acc_cp);
+      if (out_cta) { p.counters[16] = F.vt_n[0]; p.counters[17] = F.vt_n[1]; }
+      atomicAdd(&p.counters[18], vt_rows); atomicAdd(&p.counters[19], vt_fallback);
       }
 
     }
@@ -2121,3 +2257,6 @@ __global__ void __launch_bounds__(256, 1) k_commit_fast(K2Params p, FastParams f
     for (int k = 0; k < 8; ++k) p.prof[k] = S.prof[k];
   }
 }
+#undef VT
+#undef VT_AT
+#undef VT_GSTAMP

@@ -48,6 +48,10 @@ int fail(int code, const char *fmt, ...) {
 // the count all-gather of feasible-node sampling
 constexpr size_t kMbox2Offset = (size_t)MBOX_STRIDE * 2 * 2048;                // in uint4
 constexpr size_t kMboxBytes = sizeof(uint4) * MBOX_STRIDE * 2 * 2048 * 2;
+constexpr size_t kCounters = 32;  // int32 counters of the commit kernels
+// Device memory the incremental kernel may spend on its per-group verdict table (n_groups x node slots x 9 B). Sessions
+// above it are those whose requests are nearly all distinct: groups rarely recur there, and a re-entry takes a full sweep.
+constexpr size_t kVerdictTableBudget = (size_t)256 << 20;
 
 // a launch whose grid.y runs over `count` groups / work items, in slices of at most 65535 (the limit of gridDim.y)
 #define LAUNCH_Y_SLICED(kernel, gx, count, block, smem, stream, P, ...)                         \
@@ -177,6 +181,10 @@ struct vc_snapshot {
   bool fast = false;
   uint4 *ring = nullptr;
   uint4 *d_score_log = nullptr;   // [T] tagged chosen-node score per placement attempt of the run-length batches
+  uint8_t *vt_cat = nullptr;      // per-group verdict table of k_commit_fast (FastParams::vt_*), sized for vt_entries
+  double *vt_score = nullptr;
+  int32_t *vt_gstamp = nullptr;   // sized for vt_stamps
+  size_t vt_entries = 0, vt_stamps = 0;
   int last_full = 0, last_incr = 0;
   // ---- HyperNode tree (vc_snapshot_set_topology) ----
   bool has_topo = false;
@@ -428,7 +436,7 @@ void choose_geometry(vc_snapshot *s) {
     if (g_tun.commit_threads <= 0) s->block = 256;  // 7 worker warps: a run's node states are evaluated two per warp
     size_t rows = 3 * (size_t)R + (s->dc.has_future ? 2 * (size_t)R : 0) + 2 * (size_t)K + 2 + 1;
     s->smem_bytes = ((sizeof(Ctl) + 15) & ~(size_t)15) + ((sizeof(CtlFast) + 15) & ~(size_t)15) + rows * npc * 8 +
-                    (size_t)npc * (8 + 4 * 5) + (size_t)s->n_cta_total * (8 + 4 + 4 + 4 + 4) + 64;
+                    (size_t)npc * (8 + 4 * 7) + (size_t)s->n_cta_total * (8 + 4 + 4 + 4 + 4) + 64;
     const size_t heap_bytes = (size_t)s->heap_total * sizeof(HeapKey);
     s->heap_in_smem = (heap_bytes <= 96 * 1024 && s->smem_bytes + heap_bytes <= 200 * 1024) ? 1 : 0;
     if (s->heap_in_smem) s->smem_bytes += heap_bytes + 16;
@@ -525,7 +533,8 @@ void vc_snapshot_destroy(vc_snapshot *s) {
     if (r != s->rank && s->peer_comm[r]) cudaIpcCloseMemHandle(s->peer_comm[r]);
   if (s->comm) cudaFree(s->comm);
   void *dptrs[] = {s->in.dev, s->cstat, s->w_idle, s->w_used, s->w_pip, s->w_kreq, s->w_knz, s->w_pod_count,
-                   s->rep_i32, s->rep_f64, s->rep_heap, s->rep_hn_used, s->rep_placed, s->d_job_alloc, s->hn_score, s->mbox, s->ring, s->d_score_log, s->d_prof, s->d_wait, s->d_dbg, s->d_nominated, s->d_decisions, s->d_visits, s->d_fit, s->d_counters, s->d_bf, s->w_rel, s->d_ev, s->d_hd, s->rep_hd, s->d_hdp, s->d_topo};
+                   s->rep_i32, s->rep_f64, s->rep_heap, s->rep_hn_used, s->rep_placed, s->d_job_alloc, s->hn_score, s->mbox, s->ring, s->d_score_log, s->d_prof, s->d_wait, s->d_dbg, s->d_nominated, s->d_decisions, s->d_visits, s->d_fit, s->d_counters, s->d_bf, s->w_rel, s->d_ev, s->d_hd, s->rep_hd, s->d_hdp, s->d_topo,
+                   s->vt_cat, s->vt_score, s->vt_gstamp};
   for (void *p : dptrs) if (p) cudaFree(p);
   void *hptrs[] = {s->in.pin, s->h_decisions, s->h_visits, s->h_fit, s->h_counters, s->h_ev, s->delta_pin, s->h_topo};
   if (s->delta_dev) cudaFree(s->delta_dev);
@@ -1534,15 +1543,32 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   const size_t ring_bytes = sizeof(uint4) * RING_STRIDE * RING_DEPTH;
   if (!s->ring) CUDA_TRY(cudaMalloc(&s->ring, ring_bytes));
   if (!s->d_score_log) CUDA_TRY(cudaMalloc(&s->d_score_log, (T + 64) * sizeof(uint4)));
+  // per-group verdict table: every (group, node slot of this rank) when the session fits the budget (not the SOFT instance)
+  const size_t vt_entries = (size_t)s->n_groups * G * s->npc;
+  const bool vt_on = s->fast && !s->dc.soft_active && vt_entries > 0 && vt_entries * 9 <= kVerdictTableBudget;
+  if (vt_on && s->vt_entries < vt_entries) {
+    if (s->vt_cat) cudaFree(s->vt_cat);
+    if (s->vt_score) cudaFree(s->vt_score);
+    s->vt_cat = nullptr; s->vt_score = nullptr; s->vt_entries = 0;
+    CUDA_TRY(cudaMalloc(&s->vt_cat, vt_entries));
+    CUDA_TRY(cudaMalloc(&s->vt_score, vt_entries * 8));
+    s->vt_entries = vt_entries;
+  }
+  if (vt_on && s->vt_stamps < (size_t)s->n_groups * G) {
+    if (s->vt_gstamp) cudaFree(s->vt_gstamp);
+    s->vt_gstamp = nullptr; s->vt_stamps = 0;
+    CUDA_TRY(cudaMalloc(&s->vt_gstamp, (size_t)s->n_groups * G * 4));
+    s->vt_stamps = (size_t)s->n_groups * G;
+  }
   if (!s->d_decisions) {
     CUDA_TRY(cudaMalloc(&s->d_decisions, std::max<size_t>(1, T) * sizeof(vc_decision)));
     CUDA_TRY(cudaMalloc(&s->d_visits, (T + J + 1) * sizeof(vc_visit)));
     CUDA_TRY(cudaMalloc(&s->d_fit, std::max<size_t>(1, T) * 4));
-    CUDA_TRY(cudaMalloc(&s->d_counters, 16 * 4));
+    CUDA_TRY(cudaMalloc(&s->d_counters, kCounters * 4));
     CUDA_TRY(cudaMallocHost(&s->h_decisions, std::max<size_t>(1, T) * sizeof(vc_decision)));
     CUDA_TRY(cudaMallocHost(&s->h_visits, (T + J + 1) * sizeof(vc_visit)));
     CUDA_TRY(cudaMallocHost(&s->h_fit, std::max<size_t>(1, T) * 4));
-    CUDA_TRY(cudaMallocHost(&s->h_counters, 16 * 4));
+    CUDA_TRY(cudaMallocHost(&s->h_counters, kCounters * 4));
   }
   K2Params p;
   std::memset(&p, 0, sizeof p);
@@ -1647,6 +1673,9 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   fp.run_max = (s->rows_integral && !g_tun.commit_norun && s->dc.to_find == 0)
                    ? std::max(1, std::min(g_tun.run_max > 0 ? g_tun.run_max : RUN_MAX, std::min(RUN_MAX, 2 * (s->block / 32 - 1)))) : 1;
   fp.score_log = s->d_score_log;
+  fp.vt_cat = vt_on ? s->vt_cat : nullptr;
+  fp.vt_score = vt_on ? s->vt_score : nullptr;
+  fp.vt_gstamp = vt_on ? s->vt_gstamp : nullptr;
   if (s->world > 1) {  // mailbox, ring and score log live in the exported slabs; the score log is rank 0's (it writes the decisions)
     p.mbox = reinterpret_cast<uint4 *>(s->comm);
     p.ring = reinterpret_cast<uint4 *>(s->comm + s->comm_ring_off);
@@ -1665,7 +1694,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
     CUDA_TRY(cudaMemsetAsync(s->mbox, 0, mbox_bytes, s->stream));
     if (s->fast) CUDA_TRY(cudaMemsetAsync(s->d_score_log, 0, (T + 64) * sizeof(uint4), s->stream));
   }
-  CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, 16 * 4, s->stream));
+  CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, kCounters * 4, s->stream));
   // working copies of the mutable node state (the uploaded snapshot stays intact for re-runs / K1)
   CUDA_TRY(cudaMemcpyAsync(s->w_idle, s->n_idle.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
   CUDA_TRY(cudaMemcpyAsync(s->w_used, s->n_used.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
@@ -1678,7 +1707,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   CUDA_TRY(cudaLaunchCooperativeKernel(kfn, dim3(G), dim3(s->block), args, s->smem_bytes, s->stream));
   g_launches++;
   CUDA_TRY(cudaEventRecord(s->ev1, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(s->h_counters, s->d_counters, 16 * 4, cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(s->h_counters, s->d_counters, kCounters * 4, cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaMemcpyAsync(s->h_prof, s->d_prof, 16 * sizeof(long long), cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaStreamSynchronize(s->stream));
   if (d_wait) {
@@ -1753,6 +1782,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   r->stats.prof_cycles[6] = s->h_counters[5];  // full sweeps (fast kernel)
   r->stats.prof_cycles[7] = s->h_counters[6];  // incremental steps (fast kernel)
   r->stats.prof_cycles[5] = s->h_counters[7];  // owner changes between consecutive publications
+  for (int k = 0; k < 4; ++k) r->stats.group_reentry[k] = s->h_counters[16 + k];
   if (g_tun.prof_owner)
     fprintf(stderr, "runs: %d publications covering %d placements (%.2f per run), command -> publish %.0f cycles per run\n",
             s->h_counters[13], s->h_counters[14], (double)s->h_counters[14] / std::max(1, s->h_counters[13]),

@@ -159,7 +159,7 @@ class Engine:
             ja = self.L.vc_result_job_allocated_hypernodes(r, C.byref(nj))
             job_alloc = np.ctypeslib.as_array(ja, (nj.value,)).copy() if nj.value else None
             st = self.L.vc_result_stats(r).contents
-            stats = {k: (list(getattr(st, k)) if k == "prof_cycles" else getattr(st, k)) for k, _ in abi.vc_stats._fields_}
+            stats = {k: (list(getattr(st, k)) if k in ("prof_cycles", "group_reentry") else getattr(st, k)) for k, _ in abi.vc_stats._fields_}
         finally:
             self.L.vc_result_free(r)
         res = AllocateResult(dec, vis, fe, stats)
