@@ -18,8 +18,12 @@ import (
 	"unsafe"
 
 	v1 "k8s.io/api/core/v1"
+	policyv1 "k8s.io/api/policy/v1"
+	metav1 "k8s.io/apimachinery/pkg/apis/meta/v1"
+	"k8s.io/apimachinery/pkg/labels"
 	"k8s.io/klog/v2"
 
+	"volcano.sh/apis/pkg/apis/scheduling/v1beta1"
 	"volcano.sh/volcano/cmd/scheduler/app/options"
 	stockallocate "volcano.sh/volcano/pkg/scheduler/actions/allocate"
 	stockbackfill "volcano.sh/volcano/pkg/scheduler/actions/backfill"
@@ -434,6 +438,105 @@ func setPreemptOptions(ssn *framework.Session, e *session) bool {
 	return true
 }
 
+// guardsVote: pdb or cdp registers a victim function the action calls (EnabledPreemptable for preempt, EnabledReclaimable
+// for reclaim), the library's test for requiring the table. Other sessions skip the PDB list and the per-pod work.
+func guardsVote(ssn *framework.Session, action string) bool {
+	for _, tier := range ssn.Tiers {
+		for _, p := range tier.Plugins {
+			if p.Name != "pdb" && p.Name != "cdp" {
+				continue
+			}
+			en := p.EnabledPreemptable
+			if action == "reclaim" {
+				en = p.EnabledReclaimable
+			} else if action != "preempt" {
+				continue
+			}
+			if en != nil && *en {
+				return true
+			}
+		}
+	}
+	return false
+}
+
+// cooldownUntil is LastTransitionTime + cooldown in ns, saturated to the int64 range (UnixNano is undefined outside it; a
+// protection end past it stays after any now, one before it is never after now)
+func cooldownUntil(t time.Time) int64 {
+	if t.After(time.Unix(0, math.MaxInt64)) {
+		return math.MaxInt64
+	}
+	if t.Before(time.Unix(0, math.MinInt64+1)) {
+		return math.MinInt64 // VC_COOLDOWN_NONE
+	}
+	return t.UnixNano()
+}
+
+// setVictimGuards hands the library what the pdb and cdp victim votes read (vc_victim_guards): the PDBs listed through the
+// informer factory as getPodDisruptionBudgets does (pdb.go:143-153), matched per running pod with LabelSelectorAsSelector,
+// and per pod the end of cdp's cooldown (cdp.go:56-96). One time.Now() for the session.
+func setVictimGuards(ssn *framework.Session, e *session) bool {
+	n := len(e.runTasks)
+	var pdbs []*policyv1.PodDisruptionBudget
+	if f := ssn.InformerFactory(); f != nil {
+		list, err := f.Policy().V1().PodDisruptionBudgets().Lister().List(labels.Everything())
+		if err != nil {
+			fail("victim guards: pdb list")
+			return false
+		}
+		pdbs = list
+	}
+	allowed := make([]int32, len(pdbs)+1)
+	sel := make([]labels.Selector, len(pdbs))
+	for i, b := range pdbs {
+		allowed[i] = b.Status.DisruptionsAllowed
+		if s, err := metav1.LabelSelectorAsSelector(b.Spec.Selector); err == nil && !s.Empty() {
+			sel[i] = s
+		}
+	}
+	off, list := make([]int32, n+1), make([]int32, 0, n+1)
+	flags, until := make([]uint32, n+1), make([]int64, n+1)
+	for i, t := range e.runTasks {
+		pod := t.Pod
+		if len(pod.Labels) == 0 {
+			flags[i] |= C.VC_GUARD_NO_LABELS
+		} else {
+			for k, b := range pdbs {
+				if b.Namespace != pod.Namespace || sel[k] == nil || !sel[k].Matches(labels.Set(pod.Labels)) {
+					continue
+				}
+				if _, ok := b.Status.DisruptedPods[pod.Name]; ok {
+					continue
+				}
+				list = append(list, int32(k))
+			}
+		}
+		off[i+1] = int32(len(list))
+		until[i] = math.MinInt64 // VC_COOLDOWN_NONE
+		v, ok := pod.Labels[v1beta1.CooldownTime]
+		if !ok {
+			v, ok = pod.Annotations[v1beta1.CooldownTime]
+		}
+		if d, err := time.ParseDuration(v); ok && err == nil && pod.Status.Phase == v1.PodRunning {
+			for _, c := range pod.Status.Conditions {
+				if c.Type == v1.PodScheduled && c.Status == v1.ConditionTrue {
+					until[i] = cooldownUntil(c.LastTransitionTime.Add(d))
+					break
+				}
+			}
+		}
+	}
+	list = append(list, 0) // keep the slice's pointer valid when empty
+	g := C.vc_victim_guards{n_running: C.int32_t(n), n_pdb: C.int32_t(len(pdbs)), pdb_allowed: ptrI(allowed),
+		rt_pdb_off: ptrI(off), rt_pdb: ptrI(list), rt_flags: ptrU(flags), rt_cooldown_until_ns: ptrL(until),
+		now_ns: C.int64_t(time.Now().UnixNano())}
+	if rc := C.vc_snapshot_set_victim_guards(cur.snap, &g); rc != 0 {
+		fail("victim guards")
+		return false
+	}
+	return true
+}
+
 // ---- backfill / preempt / reclaim on the same device session ------------------------------------------------------------
 
 type followUp struct{ name string }
@@ -458,6 +561,10 @@ func (a *followUp) Execute(ssn *framework.Session) {
 	e := cur.enc
 	var res *C.vc_result
 	var rc C.int
+	if guardsVote(ssn, a.name) && !setVictimGuards(ssn, e) {
+		runStock(a.name, ssn)
+		return
+	}
 	switch a.name {
 	case "backfill":
 		rc = C.vc_backfill_run(cur.snap, &res)

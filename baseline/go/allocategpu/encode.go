@@ -792,7 +792,7 @@ func (e *session) encodeConf(tiers []conf.Tier, enqueueConfigured bool) {
 	ids := map[string]C.int32_t{"priority": C.VC_PLUGIN_PRIORITY, "gang": C.VC_PLUGIN_GANG, "drf": C.VC_PLUGIN_DRF,
 		"proportion": C.VC_PLUGIN_PROPORTION, "predicates": C.VC_PLUGIN_PREDICATES, "nodeorder": C.VC_PLUGIN_NODEORDER,
 		"binpack": C.VC_PLUGIN_BINPACK, "tdm": C.VC_PLUGIN_TDM, "network-topology-aware": C.VC_PLUGIN_NETWORK_TOPOLOGY_AWARE,
-		"conformance": C.VC_PLUGIN_CONFORMANCE}
+		"conformance": C.VC_PLUGIN_CONFORMANCE, "pdb": C.VC_PLUGIN_PDB, "cdp": C.VC_PLUGIN_CDP}
 	on := func(b *bool) bool { return b != nil && *b }
 	c.binpack_weight = 1
 	for d := range c.binpack_dim_weight {

@@ -52,7 +52,7 @@
 extern "C" {
 #endif
 
-#define VC_ABI_VERSION 6
+#define VC_ABI_VERSION 7
 #define VC_MAX_DIMS 16   /* R  */
 #define VC_MAX_KDIMS 4   /* dims seen by the upstream kube-scheduler scorers (cpu, memory, nvidia.com/gpu, ...) */
 #define VC_MAX_WORDS 4   /* 64-bit words per label / taint bitset */
@@ -203,7 +203,9 @@ enum vc_plugin {
   VC_PLUGIN_TDM = 8,
   VC_PLUGIN_NETWORK_TOPOLOGY_AWARE = 9,
   VC_PLUGIN_CONFORMANCE = 10, /* evictableFn: never evict critical pods (plugins/conformance/conformance.go:46-66) */
-  VC_PLUGIN_OTHER = 99 /* conformance, overcommit, ...: no effect on this path */
+  VC_PLUGIN_PDB = 11, /* PreemptableFn / ReclaimableFn: PodDisruptionBudgets (plugins/pdb/pdb.go:65-137), vc_victim_guards */
+  VC_PLUGIN_CDP = 12, /* PreemptableFn / ReclaimableFn: cooldown protection (plugins/cdp/cdp.go:56-110), vc_victim_guards */
+  VC_PLUGIN_OTHER = 99 /* overcommit, ...: no effect on this path */
 };
 /* PluginOption enable flags (conf/scheduler_conf.go:60-107); nil == false unless
    ApplyPluginConfDefaults ran (plugins/defaults.go:29-55) — the caller resolves that. */
@@ -343,6 +345,30 @@ typedef struct vc_preempt_options {
   const int64_t *rt_start_ns;             /* [n_running] Pod.Status.StartTime in ns, VC_START_TIME_UNSET when nil */
 } vc_preempt_options;
 
+/* ---- what the victim votes of the pdb and cdp plugins read per running task. The caller matches selectors and parses
+   durations; the library walks the budgets and compares the times. Determinism contract of both votes:
+   - the preemptees of one ssn.Preemptable / ssn.Reclaimable call are walked in ascending running-task index (node.Tasks);
+   - PDB status (DisruptionsAllowed, DisruptedPods) is read once, at session open;
+   - every vote starts from DisruptionsAllowed again (pdb.go:75-79): evictions earlier in the session do not use up a budget;
+   - one now_ns per session stands for every time.Now() of cdp. ---- */
+#define VC_COOLDOWN_NONE INT64_MIN /* rt_cooldown_until_ns: cdp cannot protect the pod */
+#define VC_GUARD_NO_LABELS 1u      /* rt_flags: len(pod.Labels) == 0 — pdb skips the pod, so it never returns it */
+typedef struct vc_victim_guards {
+  int32_t n_running;                    /* checked against vc_running_tasks */
+  int32_t n_pdb;                        /* PodDisruptionBudgets of the session, any order */
+  const int32_t *pdb_allowed;           /* [n_pdb] Status.DisruptionsAllowed */
+  const int32_t *rt_pdb_off;            /* [n_running + 1] CSR over rt_pdb */
+  const int32_t *rt_pdb;                /* the PDBs that count task r, each once: same namespace, a non-empty selector
+                                           (metav1.LabelSelectorAsSelector without error) that matches the labels, the pod's
+                                           name not in Status.DisruptedPods. Ignored for a task flagged VC_GUARD_NO_LABELS */
+  const uint32_t *rt_flags;             /* [n_running] VC_GUARD_* */
+  const int64_t *rt_cooldown_until_ns;  /* [n_running] LastTransitionTime of the first PodScheduled=True condition plus
+                                           the volcano.sh/cooldown-time duration (label first, then annotation, by
+                                           time.ParseDuration; an invalid label disables it), for a Running pod; else
+                                           VC_COOLDOWN_NONE. cdp protects the pod while this is after now_ns */
+  int64_t now_ns;                       /* time.Now() of the session, ns since the epoch */
+} vc_victim_guards;
+
 /* ---- results ----------------------------------------------------------------------- */
 #define VC_OP_ALLOCATE 0 /* Statement.Allocate (framework/statement.go:242-302) */
 #define VC_OP_PIPELINE 1 /* Statement.Pipeline (framework/statement.go:146-200) */
@@ -461,6 +487,12 @@ int vc_snapshot_set_running(vc_snapshot *s, const vc_running_tasks *rt, const ui
    defaults, under which the action runs its normal reading. VC_EINVAL: arrays missing with n_running > 0. The reclaim
    action ignores them. */
 int vc_snapshot_set_preempt_options(vc_snapshot *s, const vc_preempt_options *opts);
+
+/* Optional, any time before vc_preempt_run / vc_reclaim_run: the table the pdb and cdp victim votes read (see
+   vc_victim_guards). Copied; NULL clears it. VC_EINVAL: arrays missing, a bad CSR, a PDB index out of range or listed twice
+   for one task. vc_preempt_run / vc_reclaim_run return VC_EINVAL when pdb or cdp votes in the action and no table is set,
+   or when its n_running differs from vc_running_tasks. */
+int vc_snapshot_set_victim_guards(vc_snapshot *s, const vc_victim_guards *g);
 
 /* ONE session across the GPUs of a node (SURVEY §8e), one process per GPU: the exact allocate loop with the node axis cut
    over the CTAs of all ranks. Every rank uploads the same snapshot and runs the same replicated control program; a CTA's

@@ -218,6 +218,55 @@ def make_soft_case(seed):
     return tc, tiers, actions, conf
 
 
+def make_guard_case(seed):
+    """The pdb and cdp plugins: make_case's clusters (make_topo_case's in a third) widened to 2-30 nodes, running pods with
+    labels app / tier or none, 1-4 PDBs with budgets 0-3 over overlapping selectors (some pods in DisruptedPods),
+    volcano.sh/cooldown-time on a third of the running pods with PodScheduled times on both sides of the cooldown's end,
+    pdb and cdp inserted at random places in the tiers (the last voter of a tier included), feasible-node sampling in half
+    the cases. -> (TestCommonStruct, tiers, actions, conf keyword arguments)."""
+    from volcano_b200.api import BuildPDB
+    rnd = random.Random(seed * 7919 + 29)
+    topo = rnd.random() < 0.33
+    tc, tiers, actions, conf = make_topo_case(seed) if topo else (*make_case(seed), {})
+    for i in range(len(tc.Nodes), rnd.randint(max(2, len(tc.Nodes)), 30)):
+        tc.Nodes.append(BuildNode(f"n{i}", BuildResourceList(str(rnd.choice([1, 2, 3, 4])), rnd.choice(["4G", "8G", "16G"]),
+                                                               ("pods", str(rnd.choice([3, 6, 20]))))))
+    now = 10 ** 18
+    running = [p for p in tc.Pods if p.node_name]
+    for p in running:
+        if rnd.random() < 0.8:
+            p.labels = dict(p.labels)
+            p.labels["app"] = rnd.choice(["a", "b"])
+            if rnd.random() < 0.5:
+                p.labels["tier"] = rnd.choice(["x", "y"])
+        if rnd.random() < 0.35:
+            cool = rnd.choice([60, 600, 3600])
+            where = p.labels if (p.labels and rnd.random() < 0.5) else p.annotations
+            where["volcano.sh/cooldown-time"] = rnd.choice([f"{cool}s", f"{cool}s", "bogus"])
+            p.scheduled_time = now - cool * 10 ** 9 + rnd.choice([-5, 0, 5]) * 10 ** 9
+    selectors = [{"app": "a"}, {"app": "b"}, {"tier": "x"}, {"app": "a", "tier": "y"}, {}]
+    ns = tc.Pods[0].namespace if tc.Pods else "default"
+    pdbs = []
+    for i in range(rnd.randint(1, 4)):
+        disrupted = [p.name for p in running if rnd.random() < 0.1]
+        pdbs.append(BuildPDB(ns, f"pdb{i}", rnd.choice(selectors), rnd.randint(0, 3), disrupted))
+    tc.PDBs = pdbs
+    for name in ("pdb", "cdp"):
+        if rnd.random() < 0.8:
+            t = rnd.randrange(len(tiers))
+            tiers[t].insert(rnd.randint(0, len(tiers[t])), PluginOption.defaults(name))
+    if not any(o.name in ("pdb", "cdp") for t in tiers for o in t):
+        tiers[-1].append(PluginOption.defaults("pdb"))
+    actions = tuple(a for a in actions if a != "allocate" or rnd.random() < 0.5)
+    if not any(a in ("preempt", "reclaim") for a in actions):
+        actions = actions + ("preempt",)
+    conf["now_ns"] = now
+    if rnd.random() < 0.5:
+        conf.update(percentage_nodes_to_find=rnd.choice([34, 50, 67]), min_nodes_to_find=1,
+                    last_processed_node_index=rnd.randint(0, 2 * len(tc.Nodes)), enable_predicate_error_cache=False)
+    return tc, tiers, actions, conf
+
+
 def _plugins_and_actions(rnd):
     voters = [n for n in ("conformance", "gang", "priority", "drf", "proportion") if rnd.random() < 0.75]
     scorers = [n for n in ("predicates", "nodeorder", "binpack") if rnd.random() < 0.5]

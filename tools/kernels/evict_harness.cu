@@ -144,9 +144,18 @@ struct EhSoftArgs {
   unsigned long long *word;       // the reduction word after the launches
 };
 
-static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx);
+static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx, const uint8_t *guard = nullptr);
 
 extern "C" int eh_rank(const EhRankArgs *a) { return rank_run(a, nullptr); }
+
+// The GUARD instance k_evict_rank<16, .., false, true> (sessions where pdb or cdp votes): guard[RT] holds the VCT_GUARD_*
+// bits vcalloc.cu derives from the victim-guard table.
+extern "C" int eh_rank_guard(const EhRankArgs *a, const uint8_t *guard) {
+  if (!a || (a->RT > 0 && !guard)) return EH_EINVAL;
+  for (int r = 0; r < a->RT; ++r)
+    if (guard[r] & ~(VCT_GUARD_NO_LABELS | VCT_GUARD_PDB_NEVER | VCT_GUARD_CDP)) return EH_EINVAL;
+  return rank_run(a, nullptr, guard);
+}
 
 extern "C" int eh_soft_chain(const EhRankArgs *a, const EhSoftArgs *sx) {
   if (!a || !sx || !sx->order || !sx->n_order || !sx->word || a->N < 1 || a->mode == EV_MODE_RECLAIM) return EH_EINVAL;
@@ -207,7 +216,7 @@ static int soft_chain(const EhRankArgs *a, const EhSoftArgs &sx, EvictParams p, 
   return EH_OK;
 }
 
-static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx) {
+static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx, const uint8_t *guard) {
   if (!a) return EH_EINVAL;
   const int N = a->N, R = a->R, RT = a->RT, J = a->J, Q = a->Q;
   if (N < 0 || R < 2 || R > VC_MAX_DIMS || RT < 0 || J < 0 || Q < 0 || a->pods_dim < -1 || a->pods_dim >= R) return EH_EINVAL;
@@ -240,9 +249,10 @@ static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx) {
   DevBuf<double> idle, rel, pip, rt_req;
   DevBuf<uint32_t> cstat, rt_flags, q_flags;
   DevBuf<int32_t> rt_off, rt_idx, rt_job, rt_prio, j_queue, j_prio, j_min, j_ready;
-  DevBuf<uint8_t> rt_ev, q_over, cand;
+  DevBuf<uint8_t> rt_ev, q_over, cand, rt_guard;
   DevBuf<unsigned long long> key;
   const size_t RN = (size_t)R * N;
+  if (guard) EH_TRY(rt_guard.put(guard, RT));
   EH_TRY(idle.put(a->idle, RN)); EH_TRY(rel.put(a->rel, RN)); EH_TRY(pip.put(a->pip, RN));
   EH_TRY(cstat.put(a->cstat, N)); EH_TRY(rt_off.put(a->rt_off, N > 0 ? N + 1 : 0));
   EH_TRY(rt_idx.put(a->rt_idx, RT)); EH_TRY(rt_req.put(a->rt_req, (size_t)R * RT)); EH_TRY(rt_flags.put(a->rt_flags, RT));
@@ -262,6 +272,7 @@ static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx) {
   p.exact_sums = a->exact_sums ? 1 : 0;
   p.RT = RT;
   p.key = key.d; p.cand = cand.d;
+  p.rt_guard = rt_guard.d;
   EvictTask t;
   std::memset(&t, 0, sizeof t);
   for (int d = 0; d < R; ++d) t.rec.req[d] = a->req[d];
@@ -273,8 +284,14 @@ static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx) {
     for (int d = 0; d < R; ++d) { t.qalloc[d] = a->qalloc[d]; t.qdes[d] = a->qdes[d]; }
   if (sx) return soft_chain(a, *sx, p, t);
   if (N > 0) {  // the instance vcalloc.cu picks for R
-    if (R <= 8) k_evict_rank<16, 8><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);
-    else k_evict_rank<16, VC_MAX_DIMS><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);
+    const unsigned grid = (unsigned)(((size_t)N * 16 + 255) / 256);
+    if (guard) {
+      if (R <= 8) k_evict_rank<16, 8, false, true><<<grid, 256>>>(p, t);
+      else k_evict_rank<16, VC_MAX_DIMS, false, true><<<grid, 256>>>(p, t);
+    } else {
+      if (R <= 8) k_evict_rank<16, 8><<<grid, 256>>>(p, t);
+      else k_evict_rank<16, VC_MAX_DIMS><<<grid, 256>>>(p, t);
+    }
     EH_TRY(cudaGetLastError());
   }
   EH_TRY(cudaDeviceSynchronize());
@@ -342,7 +359,39 @@ extern "C" int eh_apply(const EhApplyArgs *a) {
 // ---- k_evict_dryrun / k_evict_select (topology-aware preemption) ---------------------------------------------------
 #include "topo_args.h"
 
-extern "C" int eh_dryrun(const EhTopoArgs *a) {
+// The victim-guard table of the GUARD instances, as vcalloc.cu stages it: VCT_GUARD_* bits [RT], the CSR of the PDBs
+// counting each task [RT + 1] / [pdb_off[RT]], DisruptionsAllowed [n_pdb].
+struct EhGuardArgs {
+  int n_pdb;
+  const uint8_t *bits;
+  const int32_t *pdb_off, *pdb, *pdb_allowed;
+};
+
+static int dryrun_run(const EhTopoArgs *a, const EhGuardArgs *g, const int32_t *samp_list, int n_samp);
+
+extern "C" int eh_dryrun(const EhTopoArgs *a) { return dryrun_run(a, nullptr, nullptr, 0); }
+
+// k_evict_dryrun<SAMP, true>: samp_list == nullptr runs the non-sampling instance over every predicate node; otherwise the
+// SAMP instance runs on the n_samp listed nodes (k_evict_samp's list: predicate nodes in scan order)
+extern "C" int eh_dryrun_guard(const EhTopoArgs *a, const EhGuardArgs *g, const int32_t *samp_list, int n_samp) {
+  if (!a || !g || g->n_pdb < 0 || (a->RT > 0 && (!g->bits || !g->pdb_off)) || (g->n_pdb > 0 && !g->pdb_allowed)) return EH_EINVAL;
+  if (a->RT > 0) {
+    if (g->pdb_off[0] != 0) return EH_EINVAL;
+    for (int r = 0; r < a->RT; ++r)
+      if (g->pdb_off[r + 1] < g->pdb_off[r]) return EH_EINVAL;
+    if (g->pdb_off[a->RT] > 0 && !g->pdb) return EH_EINVAL;
+    for (int x = 0; x < g->pdb_off[a->RT]; ++x)
+      if (g->pdb[x] < 0 || g->pdb[x] >= g->n_pdb) return EH_EINVAL;
+  }
+  if (samp_list) {
+    if (n_samp < 0 || n_samp > a->N) return EH_EINVAL;
+    for (int i = 0; i < n_samp; ++i)
+      if (samp_list[i] < 0 || samp_list[i] >= a->N) return EH_EINVAL;
+  }
+  return dryrun_run(a, g, samp_list, n_samp);
+}
+
+static int dryrun_run(const EhTopoArgs *a, const EhGuardArgs *g, const int32_t *samp_list, int n_samp) {
   if (!a || !eh_topo_check(*a)) return EH_EINVAL;
   const int N = a->N, R = a->R, J = a->J, RT = a->RT;
   const size_t B = (size_t)(RT > 0 ? RT : 1);
@@ -366,6 +415,13 @@ extern "C" int eh_dryrun(const EhTopoArgs *a) {
   EH_TRY(j_alloc.put(a->j_alloc, (size_t)R * J)); EH_TRY(j_share.put(a->j_share, J));
   EH_TRY(sa.put(nullptr, B)); EH_TRY(sb.put(nullptr, B)); EH_TRY(sf.put(nullptr, B)); EH_TRY(sg.put(nullptr, B));
   EH_TRY(ok.put(nullptr, N)); EH_TRY(nv.put(nullptr, N)); EH_TRY(key.put(nullptr, 4 * (size_t)N));
+  DevBuf<uint8_t> g_bits;
+  DevBuf<int32_t> g_off, g_pdb, g_allowed, d_list, d_cnt;
+  if (g) {
+    EH_TRY(g_bits.put(g->bits, RT)); EH_TRY(g_off.put(g->pdb_off, RT > 0 ? (size_t)RT + 1 : 0));
+    EH_TRY(g_pdb.put(g->pdb, RT > 0 ? (size_t)g->pdb_off[RT] : 0)); EH_TRY(g_allowed.put(g->pdb_allowed, g->n_pdb));
+  }
+  if (samp_list) { EH_TRY(d_list.put(samp_list, n_samp)); EH_TRY(d_cnt.put(&n_samp, 1)); }
   vct::TopoView v;
   std::memset(&v, 0, sizeof v);
   v.R = R; v.N = N; v.J = J; v.RT = RT; v.pods_dim = a->pods_dim; v.n_plugins = a->n_plugins;
@@ -378,12 +434,17 @@ extern "C" int eh_dryrun(const EhTopoArgs *a) {
   v.j_rank = j_rank.d; v.j_alloc = j_alloc.d; v.j_share = j_share.d;
   for (int d = 0; d < R; ++d) v.total[d] = a->total[d];
   v.total_has = a->total_has;
+  v.rt_guard = g_bits.d; v.pdb_off = g_off.d; v.pdb = g_pdb.d; v.pdb_allowed = g_allowed.d;
   vct::TopoTask t;
   eh_topo_task(*a, t);
   TopoDry s;
   s.cstat = cstat.d; s.klass = 0; s.a = sa.d; s.b = sb.d; s.f = sf.d; s.g = sg.d; s.ok = ok.d; s.nv = nv.d; s.key = key.d;
+  s.samp_list = d_list.d; s.samp_cnt = d_cnt.d;
   if (N > 0) {  // the production geometry (vcalloc.cu)
-    k_evict_dryrun<false><<<(unsigned)((N + 127) / 128), 128>>>(v, t, s);
+    const unsigned grid = (unsigned)((N + 127) / 128);
+    if (!g) k_evict_dryrun<false><<<grid, 128>>>(v, t, s);
+    else if (!samp_list) k_evict_dryrun<false, true><<<grid, 128>>>(v, t, s);
+    else if (n_samp > 0) k_evict_dryrun<true, true><<<grid, 128>>>(v, t, s);
     EH_TRY(cudaGetLastError());
   }
   EH_TRY(cudaDeviceSynchronize());

@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 
-VC_ABI_VERSION = 6
+VC_ABI_VERSION = 7
 VC_MAX_DIMS = 16
 VC_MAX_KDIMS = 4
 VC_MAX_WORDS = 4
@@ -45,6 +45,8 @@ VC_PLUGIN_BINPACK = 7
 VC_PLUGIN_TDM = 8
 VC_PLUGIN_NETWORK_TOPOLOGY_AWARE = 9
 VC_PLUGIN_CONFORMANCE = 10
+VC_PLUGIN_PDB = 11
+VC_PLUGIN_CDP = 12
 VC_PLUGIN_OTHER = 99
 PLUGIN_IDS = {
     "priority": VC_PLUGIN_PRIORITY,
@@ -57,6 +59,8 @@ PLUGIN_IDS = {
     "tdm": VC_PLUGIN_TDM,
     "network-topology-aware": VC_PLUGIN_NETWORK_TOPOLOGY_AWARE,
     "conformance": VC_PLUGIN_CONFORMANCE,
+    "pdb": VC_PLUGIN_PDB,
+    "cdp": VC_PLUGIN_CDP,
 }
 
 VC_EN_JOB_ORDER = 0x001
@@ -220,6 +224,15 @@ class vc_preempt_options(C.Structure):
                 ("rt_pod_priority", _i32p), ("rt_start_ns", _i64p)]
 
 
+VC_COOLDOWN_NONE = -(2 ** 63)
+VC_GUARD_NO_LABELS = 1
+
+
+class vc_victim_guards(C.Structure):
+    _fields_ = [("n_running", C.c_int32), ("n_pdb", C.c_int32), ("pdb_allowed", _i32p), ("rt_pdb_off", _i32p),
+                ("rt_pdb", _i32p), ("rt_flags", _u32p), ("rt_cooldown_until_ns", _i64p), ("now_ns", C.c_int64)]
+
+
 class vc_decision(C.Structure):
     _fields_ = [("task", C.c_int32), ("node", C.c_int32), ("kind", C.c_int32), ("visit", C.c_int32),
                 ("score", C.c_double)]
@@ -258,6 +271,7 @@ SYMBOLS = {
     "vc_snapshot_set_running": (C.c_int, [_vp, C.POINTER(vc_running_tasks), C.POINTER(C.c_uint32)]),
     "vc_snapshot_set_nominated": (C.c_int, [_vp, C.POINTER(C.c_int32)]),
     "vc_snapshot_set_preempt_options": (C.c_int, [_vp, C.POINTER(vc_preempt_options)]),
+    "vc_snapshot_set_victim_guards": (C.c_int, [_vp, C.POINTER(vc_victim_guards)]),
     "vc_comm_create": (C.c_int, [_vp, C.c_int, C.c_int, C.c_void_p]),
     "vc_comm_attach": (C.c_int, [_vp, C.c_void_p]),
     "vc_comm_prepare": (C.c_int, [_vp]),

@@ -189,6 +189,7 @@ class Pod:
     priority_class_name: str = ""  # pod.Spec.PriorityClassName (conformance: system-*-critical pods are never evicted)
     nominated_node_name: str = ""  # pod.Status.NominatedNodeName (left by a preemption of an earlier cycle, allocate.go:624-634)
     start_time: Optional[int] = None  # pod.Status.StartTime in ns since the epoch (None: not started)
+    scheduled_time: Optional[int] = None  # LastTransitionTime of the first PodScheduled=True condition, ns (None: none)
 
     def __post_init__(self):
         if not self.uid:
@@ -249,6 +250,83 @@ class HyperNode:
 
 def BuildHyperNode(name: str, tier: int, members: Sequence[Tuple[str, str]]) -> HyperNode:
     return HyperNode(name=name, tier=tier, members=[(m[0], m[1]) for m in members])
+
+
+@dataclass
+class PodDisruptionBudget:
+    """policy/v1 PodDisruptionBudget as the pdb plugin reads it (plugins/pdb/pdb.go:65-126): the selector's matchLabels
+    (None or empty: a nil or empty selector, which matches nothing), Status.DisruptionsAllowed and the names in
+    Status.DisruptedPods."""
+    namespace: str
+    name: str
+    match_labels: Optional[Dict[str, str]] = None
+    disruptions_allowed: int = 0
+    disrupted_pods: List[str] = field(default_factory=list)
+
+    def counts(self, pod: "Pod") -> bool:
+        """Whether this PDB takes one from its budget when the plugin walks `pod` (a pod with labels)."""
+        return (self.namespace == pod.namespace and bool(self.match_labels)
+                and all(pod.labels.get(k) == v for k, v in self.match_labels.items())
+                and pod.name not in self.disrupted_pods)
+
+
+def BuildPDB(namespace: str, name: str, match_labels: Optional[Dict[str, str]], disruptions_allowed: int,
+             disrupted_pods: Sequence[str] = ()) -> PodDisruptionBudget:
+    return PodDisruptionBudget(namespace, name, dict(match_labels) if match_labels is not None else None,
+                               disruptions_allowed, list(disrupted_pods))
+
+
+COOLDOWN_TIME_KEY = "volcano.sh/cooldown-time"  # v1beta1.CooldownTime
+
+_DURATION_UNITS = {"ns": 1, "us": 1000, "\u00b5s": 1000, "\u03bcs": 1000, "ms": 10 ** 6, "s": 10 ** 9, "m": 60 * 10 ** 9,
+                   "h": 3600 * 10 ** 9}
+_DURATION_RE = re.compile(r"([0-9]*(?:\.[0-9]*)?)([a-z\u00b5\u03bc]+)")
+
+
+def go_parse_duration(text: str) -> Optional[int]:
+    """time.ParseDuration in ns, None where it returns an error."""
+    s = text
+    neg = False
+    if s[:1] in ("-", "+"):
+        neg, s = s[0] == "-", s[1:]
+    if s == "0":
+        return 0
+    if not s:
+        return None
+    total, pos = 0, 0
+    while pos < len(s):
+        m = _DURATION_RE.match(s, pos)
+        if not m or m.group(1) in ("", ".") or m.group(2) not in _DURATION_UNITS:
+            return None
+        whole, _, frac = m.group(1).partition(".")
+        unit = _DURATION_UNITS[m.group(2)]
+        v = int(whole or "0") * unit
+        if frac:
+            scale = 1
+            f = 0
+            for ch in frac:  # the fraction is truncated to whole nanoseconds, as Go's leadingFraction + float scaling
+                if scale >= 10 ** 18:
+                    break
+                f = f * 10 + int(ch)
+                scale *= 10
+            v += int(f * (unit / scale))
+        total += v
+        if total > 2 ** 63 - 1 + (1 if neg else 0):
+            return None
+        pos = m.end()
+    return -total if neg else total
+
+
+def pod_cooldown_until(pod: "Pod") -> Optional[int]:
+    """cdp's protection end (plugins/cdp/cdp.go:56-96): the cooldown from the label, else the annotation (an unparsable
+    label disables it); only a Running pod with a PodScheduled=True condition is protected; None: never protected."""
+    v = pod.labels.get(COOLDOWN_TIME_KEY, pod.annotations.get(COOLDOWN_TIME_KEY))
+    if v is None:
+        return None
+    d = go_parse_duration(v)
+    if d is None or pod.phase != "Running" or pod.scheduled_time is None:
+        return None
+    return pod.scheduled_time + d
 
 
 TASK_SPEC_KEY = "volcano.sh/task-spec"  # batch.TaskSpecKey

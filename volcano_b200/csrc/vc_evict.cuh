@@ -74,6 +74,8 @@ struct EvictParams {
   unsigned long long *soft_word;
   unsigned long long soft_seq;
   int soft_klass, soft_reduce;
+  // GUARD instances (pdb or cdp votes in the action): vct::VCT_GUARD_* bits per running task
+  const uint8_t *rt_guard;
 };
 
 struct EvNodeView {
@@ -129,7 +131,10 @@ __device__ __forceinline__ bool ev_filter(const EvictParams &p, const EvictTask 
 // replaces it — so all that is certain about a victim is that it passed the LAST voting plugin of the tier that decided.
 // Used here, per voter, is the part of its test that does not depend on the other candidates: conformance (not critical),
 // gang (job above minAvailable, gang.go:97-129), priority (lower job / task priority, priority.go:110-148), proportion
-// (queue above deserved, proportion.go:286-317); drf's test depends on the walk and counts as a yes.
+// (queue above deserved, proportion.go:286-317); drf's test depends on the walk and counts as a yes. GUARD: cdp (cooldown
+// over, exact) and pdb (labelled, and no PDB counting the task allows zero disruptions: the first decrement of such a
+// budget already protects it).
+template <bool GUARD = false>
 __device__ __forceinline__ bool ev_may_be_victim(const EvictParams &p, const EvictTask &t, int r) {
   const bool reclaim = t.mode == EV_MODE_RECLAIM;
   const uint32_t flag = reclaim ? VC_EN_RECLAIMABLE : VC_EN_PREEMPTABLE;
@@ -147,6 +152,8 @@ __device__ __forceinline__ bool ev_may_be_victim(const EvictParams &p, const Evi
       else if (pl == VC_PLUGIN_PRIORITY && !reclaim) vote = j >= 0 && (j != t.job ? p.j_prio[j] < t.job_prio : p.rt_prio[r] < t.task_prio);
       else if (pl == VC_PLUGIN_DRF && !reclaim) vote = j >= 0;
       else if (pl == VC_PLUGIN_PROPORTION && reclaim) vote = j >= 0 && p.j_queue[j] >= 0 && p.q_over[p.j_queue[j]];
+      else if (GUARD && pl == VC_PLUGIN_PDB) vote = !(p.rt_guard[r] & VCT_GUARD_PDB_NEVER);
+      else if (GUARD && pl == VC_PLUGIN_CDP) vote = !(p.rt_guard[r] & VCT_GUARD_CDP);
       else continue;
       any = true;
       last = vote;
@@ -162,7 +169,8 @@ __device__ __forceinline__ bool ev_may_be_victim(const EvictParams &p, const Evi
 // The group's first lane scores the node when it is a candidate. RMAX bounds the resource dimensions (register budget).
 // SOFT: the key is the order part only, and with soft_reduce every node passing the static predicate (candidate or not:
 // predicateNodes, scheduler_helper.go:76-136) enters the soft-taint maximum, one warp max and at most one atomic per warp.
-template <int LPN, int RMAX, bool SOFT = false>
+// GUARD: the pdb and cdp votes take part in ev_may_be_victim.
+template <int LPN, int RMAX, bool SOFT = false, bool GUARD = false>
 __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) {
   const size_t gid = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   const int n = (int)(gid / LPN);
@@ -180,7 +188,7 @@ __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) 
       const int r = p.rt_idx[k];
       if (!ev_filter(p, t, r)) continue;
       n_pass += 1;
-      if (!ev_may_be_victim(p, t, r)) continue;
+      if (!ev_may_be_victim<GUARD>(p, t, r)) continue;
 #pragma unroll
       for (int d = 0; d < RMAX; ++d)
         if (d < R) freed[d] += p.rt_req[(size_t)d * p.RT + r];
@@ -442,7 +450,7 @@ __global__ void k_evict_apply(EvictParams p, EvictTask t, int undo) {
 // ---- topology-aware preemption (vc_topo.hpp) -----------------------------------------------------------------------
 // k_evict_dryrun: SelectVictimsOnNode as a dry run on every node that passes the preemptor's predicates, one thread per
 // node. Node n's scratch is [rt_off[n], rt_off[n+1]) of four slabs over the running tasks, so a node may run any number
-// of pods; its victims stay in slab a for k_evict_select.
+// of pods; its victims stay in slab a for k_evict_select. GUARD: the pdb and cdp plugins vote (vct::topo_vote).
 struct TopoDry {
   const uint32_t *cstat;  // [C][N]
   int klass;
@@ -453,7 +461,7 @@ struct TopoDry {
   long long *key;         // [4][N] pickOneNodeForPreemption's scores
   const int32_t *samp_list, *samp_cnt;  // SAMP: thread i runs on the i-th sampled node
 };
-template <bool SAMP>
+template <bool SAMP, bool GUARD = false>
 __global__ void __launch_bounds__(128) k_evict_dryrun(vct::TopoView v, vct::TopoTask t, TopoDry s) {
   int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (SAMP) {
@@ -465,7 +473,7 @@ __global__ void __launch_bounds__(128) k_evict_dryrun(vct::TopoView v, vct::Topo
   uint8_t ok = 0;
   if (SAMP || (s.cstat[(size_t)s.klass * v.N + n] & CS_STATIC_OK)) {
     const int o = v.rt_off[n];
-    const vct::TopoResult r = vct::topo_dry_run(v, t, n, s.a + o, s.b + o, s.f + o, s.g + o);
+    const vct::TopoResult r = vct::topo_dry_run<GUARD>(v, t, n, s.a + o, s.b + o, s.f + o, s.g + o);
     ok = (uint8_t)r.ok;
     s.nv[n] = r.nv;
     for (int k = 0; k < 4; ++k) s.key[(size_t)k * v.N + n] = r.key[k];

@@ -9,6 +9,7 @@
 #include <utility>
 
 #include "vc_host.hpp"
+#include "vc_topo.hpp"
 
 namespace vch {
 
@@ -18,6 +19,24 @@ struct RunningTasks {  // host copy of vc_running_tasks + CSR over nodes
   std::vector<int64_t> podidx, ts;
   std::vector<uint32_t> uid, has, flags;
   std::vector<double> req, kreq, knz;  // [R][n], [K][n], [K][n]
+};
+
+struct VictimGuards {  // host copy of vc_victim_guards (the pdb and cdp victim votes)
+  int n_running = 0;
+  std::vector<int32_t> allowed, off, pdb;
+  std::vector<uint32_t> flags;
+  std::vector<int64_t> until;
+  int64_t now_ns = 0;
+  bool cdp_protects(int r) const { return until[r] != VC_COOLDOWN_NONE && until[r] > now_ns; }  // cdp.go:87-96
+  // the VCT_GUARD_* bits the device votes read for task r
+  uint8_t device_bits(int r) const {
+    uint8_t b = 0;
+    if (flags[r] & VC_GUARD_NO_LABELS) b |= VCT_GUARD_NO_LABELS | VCT_GUARD_PDB_NEVER;
+    for (int x = off[r]; x < off[r + 1]; ++x)
+      if (allowed[pdb[x]] <= 0) b |= VCT_GUARD_PDB_NEVER;  // the first decrement already protects the task
+    if (cdp_protects(r)) b |= VCT_GUARD_CDP;
+    return b;
+  }
 };
 
 struct EvictKeep {  // session-open state kept at every upload
@@ -111,6 +130,7 @@ struct EvictSession {
   const EvictKeep *k = nullptr;
   const RunningTasks *rt = nullptr;
   const std::vector<uint32_t> *t_flags = nullptr;
+  const VictimGuards *g = nullptr;  // set when pdb or cdp votes in the action
   int R = 0, K = 0, N = 0, T = 0, J = 0, Q = 0, pods_dim = -1;
   double total[VC_MAX_DIMS] = {0};
   uint32_t total_has = 0;
@@ -456,6 +476,24 @@ struct EvictSession {
     }
     return out;
   }
+  // pdb.go:65-126: budgets start from DisruptionsAllowed on every call; each PDB counting a labelled candidate loses one,
+  // and a candidate that drives one of them below zero is kept
+  std::vector<int> pdb_victims(const std::vector<int> &c) const {
+    std::vector<int> out;
+    std::vector<std::pair<int, int>> budget;  // PDB -> what is left of its budget in this call
+    for (int r : c) {
+      if (g->flags[r] & VC_GUARD_NO_LABELS) continue;
+      bool violated = false;
+      for (int x = g->off[r]; x < g->off[r + 1]; ++x) {
+        int *b = nullptr;
+        for (auto &e : budget) if (e.first == g->pdb[x]) b = &e.second;
+        if (!b) { budget.push_back({g->pdb[x], g->allowed[g->pdb[x]]}); b = &budget.back().second; }
+        if (--*b < 0) violated = true;
+      }
+      if (!violated) out.push_back(r);
+    }
+    return out;
+  }
   // ssn.Preemptable / ssn.Reclaimable, session_plugins.go:211-307
   std::vector<int> tier_victims(int t, const std::vector<int> &c, bool reclaim) const {
     std::vector<int> victims;
@@ -472,6 +510,8 @@ struct EvictSession {
         else if (pl == VC_PLUGIN_PRIORITY && !reclaim) cand = priority_victims(t, c);
         else if (pl == VC_PLUGIN_DRF && !reclaim) cand = drf_victims(t, c);
         else if (pl == VC_PLUGIN_PROPORTION && reclaim) cand = proportion_victims(c);
+        else if (pl == VC_PLUGIN_PDB) cand = pdb_victims(c);
+        else if (pl == VC_PLUGIN_CDP) { for (int r : c) if (!g->cdp_protects(r)) cand.push_back(r); }
         else continue;
         if (cand.empty()) { victims.clear(); nil = true; break; }
         if (nil) { victims = cand; nil = false; }

@@ -73,7 +73,13 @@ struct TopoView {  // the session as the dry run reads it; all pointers in one a
   const double *j_alloc, *j_share;         // drf: [R][J] attr.allocated, [J] attr.share
   double total[VC_MAX_DIMS];               // drf.totalResource
   uint32_t total_has;
+  // GUARD instances (pdb / cdp vote): vc_victim_guards on the device
+  const uint8_t *rt_guard;                 // [RT] VCT_GUARD_* bits
+  const int32_t *pdb_off, *pdb, *pdb_allowed;  // its CSR of the PDBs counting each task, DisruptionsAllowed per PDB
 };
+#define VCT_GUARD_NO_LABELS 1  // pdb skips the pod (pdb.go:87-90)
+#define VCT_GUARD_PDB_NEVER 2  // no labels, or a PDB with DisruptionsAllowed <= 0 counts it: pdb never returns it
+#define VCT_GUARD_CDP 4        // cdp protects it: cooldown-until after now (cdp.go:87-96)
 
 struct TopoTask {  // the preemptor and what the simulate hooks start from
   int job, queue, intra;                   // intra: victims from the preemptor's own job (preempt.go:252-268)
@@ -113,7 +119,27 @@ VC_HD double topo_drf_share(const TopoView &v, const double *a) {  // drf.calcul
   }
   return res;
 }
+// pdb.go:83-124 for candidate a[i]: it is returned unless, for some PDB counting it, the labelled candidates a[0..i] counted
+// by that PDB outnumber its DisruptionsAllowed (the budget of the call went below zero at a[i]). Counting needs no state, so
+// the dry run's scratch stays one slab entry per task of the node whatever the number of PDBs.
+VC_HD bool topo_pdb_returns(const TopoView &v, const int32_t *a, int i) {
+  const int r = a[i];
+  if (v.rt_guard[r] & VCT_GUARD_NO_LABELS) return false;
+  for (int x = v.pdb_off[r]; x < v.pdb_off[r + 1]; ++x) {
+    const int q = v.pdb[x];
+    int left = v.pdb_allowed[q];
+    for (int k = 0; k <= i && left >= 0; ++k) {
+      const int rk = a[k];
+      if (v.rt_guard[rk] & VCT_GUARD_NO_LABELS) continue;
+      for (int y = v.pdb_off[rk]; y < v.pdb_off[rk + 1]; ++y)
+        if (v.pdb[y] == q) { left -= 1; break; }
+    }
+    if (left < 0) return false;
+  }
+  return true;
+}
 // one voter of ssn.Preemptable over the candidates a[0..m): g[i] = 1 when it returns a[i]; -> number returned
+template <bool GUARD = false>
 VC_HD int topo_vote(const TopoView &v, const TopoTask &t, int pl, const int32_t *a, int m, uint8_t *g) {
   int cnt = 0;
   double ls = 0;
@@ -127,6 +153,10 @@ VC_HD int topo_vote(const TopoView &v, const TopoTask &t, int pl, const int32_t 
     bool y = false;
     if (pl == VC_PLUGIN_CONFORMANCE) {  // conformance.go:46-63
       y = !(v.rt_flags[r] & VC_RT_CRITICAL);
+    } else if (GUARD && pl == VC_PLUGIN_CDP) {
+      y = !(v.rt_guard[r] & VCT_GUARD_CDP);
+    } else if (GUARD && pl == VC_PLUGIN_PDB) {
+      y = !(v.rt_guard[r] & VCT_GUARD_PDB_NEVER) && topo_pdb_returns(v, a, i);
     } else if (j < 0) {
       y = false;
     } else if (pl == VC_PLUGIN_GANG) {  // gang.go:97-129: the job's occupancy drops with every victim it gave
@@ -211,7 +241,9 @@ VC_HD bool topo_fits(const TopoView &v, const TopoTask &t, int n, const double *
 }
 
 // SelectVictimsOnNode (preempt.go:708-842) on node n. a, b: int scratch, f, g: byte scratch, each with room for the
-// node's tasks. On success the victims are a[0..nv) in the reference's list order (reprieve order).
+// node's tasks. On success the victims are a[0..nv) in the reference's list order (reprieve order). GUARD: the pdb and cdp
+// plugins vote too.
+template <bool GUARD = false>
 VC_HD TopoResult topo_dry_run(const TopoView &v, const TopoTask &t, int n, int32_t *a, int32_t *b, uint8_t *f, uint8_t *g) {
   TopoResult res;
   res.ok = 0; res.nv = 0;
@@ -228,8 +260,10 @@ VC_HD TopoResult topo_dry_run(const TopoView &v, const TopoTask &t, int n, int32
     for (int x = i; x < v.n_plugins && v.tier[x] == tier; ++x) {
       if (!(v.enabled[x] & VC_EN_PREEMPTABLE)) continue;
       const int pl = v.plugin[x];
-      if (pl != VC_PLUGIN_GANG && pl != VC_PLUGIN_CONFORMANCE && pl != VC_PLUGIN_PRIORITY && pl != VC_PLUGIN_DRF) continue;
-      if (topo_vote(v, t, pl, a, m, g) == 0) { nil = true; break; }
+      if (pl != VC_PLUGIN_GANG && pl != VC_PLUGIN_CONFORMANCE && pl != VC_PLUGIN_PRIORITY && pl != VC_PLUGIN_DRF &&
+          !(GUARD && (pl == VC_PLUGIN_PDB || pl == VC_PLUGIN_CDP)))
+        continue;
+      if (topo_vote<GUARD>(v, t, pl, a, m, g) == 0) { nil = true; break; }
       int left = 0;
       for (int k = 0; k < m; ++k) {
         f[k] = nil ? g[k] : (uint8_t)(f[k] & g[k]);

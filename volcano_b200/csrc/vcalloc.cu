@@ -301,6 +301,11 @@ struct vc_snapshot {
   void *d_topo = nullptr;          // device slab: running-task keys, drf job state, per-node dry-run results and scratch
   size_t d_topo_bytes = 0;
   int32_t *h_topo = nullptr;       // mapped pinned: k_evict_select's hand-out, EV_TOPO_SEQ = its sequence word
+  // the pdb and cdp votes' table (vc_snapshot_set_victim_guards) and its device copy
+  bool guards_set = false;
+  vch::VictimGuards guards;
+  void *d_guard = nullptr;
+  size_t d_guard_bytes = 0;
   // ---- one session across the GPUs of a node (vc_comm_create / vc_comm_attach) ----
   int world = 1, rank = 0;
   int n_cta_total = 0;             // CTAs of all ranks (the exchange); n_cta stays this rank's grid
@@ -533,7 +538,7 @@ void vc_snapshot_destroy(vc_snapshot *s) {
     if (r != s->rank && s->peer_comm[r]) cudaIpcCloseMemHandle(s->peer_comm[r]);
   if (s->comm) cudaFree(s->comm);
   void *dptrs[] = {s->in.dev, s->cstat, s->w_idle, s->w_used, s->w_pip, s->w_kreq, s->w_knz, s->w_pod_count,
-                   s->rep_i32, s->rep_f64, s->rep_heap, s->rep_hn_used, s->rep_placed, s->d_job_alloc, s->hn_score, s->mbox, s->ring, s->d_score_log, s->d_prof, s->d_wait, s->d_dbg, s->d_nominated, s->d_decisions, s->d_visits, s->d_fit, s->d_counters, s->d_bf, s->w_rel, s->d_ev, s->d_hd, s->rep_hd, s->d_hdp, s->d_topo,
+                   s->rep_i32, s->rep_f64, s->rep_heap, s->rep_hn_used, s->rep_placed, s->d_job_alloc, s->hn_score, s->mbox, s->ring, s->d_score_log, s->d_prof, s->d_wait, s->d_dbg, s->d_nominated, s->d_decisions, s->d_visits, s->d_fit, s->d_counters, s->d_bf, s->w_rel, s->d_ev, s->d_hd, s->rep_hd, s->d_hdp, s->d_topo, s->d_guard,
                    s->vt_cat, s->vt_score, s->vt_gstamp};
   for (void *p : dptrs) if (p) cudaFree(p);
   void *hptrs[] = {s->in.pin, s->h_decisions, s->h_visits, s->h_fit, s->h_counters, s->h_ev, s->delta_pin, s->h_topo};
@@ -1863,6 +1868,38 @@ int vc_snapshot_set_preempt_options(vc_snapshot *s, const vc_preempt_options *op
   return VC_OK;
 }
 
+int vc_snapshot_set_victim_guards(vc_snapshot *s, const vc_victim_guards *g) {
+  if (!s) return fail(VC_EINVAL, "null snapshot");
+  s->guards_set = false;
+  s->guards = vch::VictimGuards();
+  if (!g) return VC_OK;
+  const int n = g->n_running, np = g->n_pdb;
+  if (n < 0 || np < 0) return fail(VC_EINVAL, "victim guards: negative sizes");
+  if ((np > 0 && !g->pdb_allowed) || !g->rt_pdb_off || (n > 0 && (!g->rt_flags || !g->rt_cooldown_until_ns)))
+    return fail(VC_EINVAL, "victim guards: arrays missing");
+  if (g->rt_pdb_off[0] != 0) return fail(VC_EINVAL, "victim guards: rt_pdb_off[0] != 0");
+  for (int r = 0; r < n; ++r)
+    if (g->rt_pdb_off[r + 1] < g->rt_pdb_off[r]) return fail(VC_EINVAL, "victim guards: rt_pdb_off decreases at %d", r);
+  const int ne = g->rt_pdb_off[n];
+  if (ne > 0 && !g->rt_pdb) return fail(VC_EINVAL, "victim guards: rt_pdb missing");
+  std::vector<int> seen((size_t)np, -1);  // a PDB counts a task once (pdb.go:92-117 visits every PDB once per task)
+  for (int r = 0; r < n; ++r)
+    for (int x = g->rt_pdb_off[r]; x < g->rt_pdb_off[r + 1]; ++x) {
+      const int q = g->rt_pdb[x];
+      if (q < 0 || q >= np) return fail(VC_EINVAL, "victim guards: task %d names PDB %d of %d", r, q, np);
+      if (seen[q] == r) return fail(VC_EINVAL, "victim guards: task %d lists PDB %d twice", r, q);
+      seen[q] = r;
+    }
+  vch::VictimGuards &h = s->guards;
+  h.n_running = n; h.now_ns = g->now_ns;
+  if (np) h.allowed.assign(g->pdb_allowed, g->pdb_allowed + np);
+  h.off.assign(g->rt_pdb_off, g->rt_pdb_off + n + 1);
+  if (ne) h.pdb.assign(g->rt_pdb, g->rt_pdb + ne);
+  if (n) { h.flags.assign(g->rt_flags, g->rt_flags + n); h.until.assign(g->rt_cooldown_until_ns, g->rt_cooldown_until_ns + n); }
+  s->guards_set = true;
+  return VC_OK;
+}
+
 namespace {
 
 // session state of the evicting actions: the opening session plus whatever vc_allocate_run did
@@ -1980,6 +2017,13 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     return fail(VC_EUNSUPPORTED, "preempt: a pending task carries a NominatedNodeName (taskEligibleToPreempt's rules are not modelled)");
   if (s->hd_set)
     return fail(VC_EUNSUPPORTED, "preempt / reclaim with drf's enableHierarchy: the hdrf tree on evict events and hdrf's reclaimFn (drf.go:280-367) are not built");
+  // pdb / cdp in ssn.Preemptable / ssn.Reclaimable read the victim-guard table
+  const bool guard_on = vch::plugin_enabled(s->conf, VC_PLUGIN_PDB, reclaim ? VC_EN_RECLAIMABLE : VC_EN_PREEMPTABLE) ||
+                        vch::plugin_enabled(s->conf, VC_PLUGIN_CDP, reclaim ? VC_EN_RECLAIMABLE : VC_EN_PREEMPTABLE);
+  if (guard_on && !s->guards_set)
+    return fail(VC_EINVAL, "%s: the pdb / cdp plugin votes and no victim-guard table is set", reclaim ? "reclaim" : "preempt");
+  if (guard_on && s->guards.n_running != s->rt.n)
+    return fail(VC_EINVAL, "victim guards: %d tasks for %d running tasks", s->guards.n_running, s->rt.n);
   const double t0 = now_ms();
   int rc = ensure_evict_session(s);
   if (rc) return rc;
@@ -1988,6 +2032,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   vch::EvictSession &e = s->es;
   const vch::EvictKeep &k = s->ek;
   const size_t B = (size_t)std::max(s->rt.n, 1);
+  e.g = guard_on ? &s->guards : nullptr;
   // device parameter block (same slab layout as ensure_evict_session)
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
@@ -2016,6 +2061,34 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     p.exact_sums = (s->rows_integral && vch::max_abs_integral(s->rt.req.data(), s->rt.req.size(), m1) &&
                     vch::max_abs_integral(k.t_req.data(), k.t_req.size(), m2) && m1 * 4096.0 < 9.0e15) ? 1 : 0;
   }
+  // the guard table on the device: per task the VCT_GUARD_* bits, then the PDB CSR and the budgets
+  const uint8_t *d_rt_guard = nullptr;
+  const int32_t *d_pdb_off = nullptr, *d_pdb = nullptr, *d_pdb_allowed = nullptr;
+  if (guard_on) {
+    const vch::VictimGuards &g = s->guards;
+    std::vector<uint8_t> bits(B, 0);
+    for (int r = 0; r < g.n_running; ++r) bits[r] = g.device_bits(r);
+    size_t goff = 0;
+    auto gtake = [&](size_t bytes) { size_t o = goff; goff = (goff + bytes + 255) & ~(size_t)255; return o; };
+    const size_t g_bits = gtake(B), g_off = gtake((B + 1) * 4), g_pdb = gtake(std::max<size_t>(g.pdb.size(), 1) * 4),
+                 g_allowed = gtake(std::max<size_t>(g.allowed.size(), 1) * 4);
+    if (goff > s->d_guard_bytes) {
+      if (s->d_guard) cudaFree(s->d_guard);
+      s->d_guard = nullptr;
+      CUDA_TRY(cudaMalloc(&s->d_guard, goff));
+      s->d_guard_bytes = goff;
+    }
+    unsigned char *gb = reinterpret_cast<unsigned char *>(s->d_guard);
+    CUDA_TRY(cudaMemcpyAsync(gb + g_bits, bits.data(), B, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(gb + g_off, g.off.data(), g.off.size() * 4, cudaMemcpyHostToDevice, s->stream));
+    if (!g.pdb.empty()) CUDA_TRY(cudaMemcpyAsync(gb + g_pdb, g.pdb.data(), g.pdb.size() * 4, cudaMemcpyHostToDevice, s->stream));
+    if (!g.allowed.empty())
+      CUDA_TRY(cudaMemcpyAsync(gb + g_allowed, g.allowed.data(), g.allowed.size() * 4, cudaMemcpyHostToDevice, s->stream));
+    d_rt_guard = gb + g_bits;
+    d_pdb_off = reinterpret_cast<const int32_t *>(gb + g_off); d_pdb = reinterpret_cast<const int32_t *>(gb + g_pdb);
+    d_pdb_allowed = reinterpret_cast<const int32_t *>(gb + g_allowed);
+  }
+  p.rt_guard = d_rt_guard;
   // topology-aware preemption: the dry run's inputs beyond the ranking's, its per-node results and scratch
   const bool topo_on = !reclaim && s->popt.topology_aware;
   vct::TopoView tv;
@@ -2071,6 +2144,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     tv.j_alloc = d_jalloc; tv.j_share = d_jshare;
     for (size_t d = 0; d < R; ++d) tv.total[d] = e.total[d];
     tv.total_has = e.total_has;
+    tv.rt_guard = d_rt_guard; tv.pdb_off = d_pdb_off; tv.pdb = d_pdb; tv.pdb_allowed = d_pdb_allowed;
     tdry.cstat = s->cstat;
     tdry.a = reinterpret_cast<int32_t *>(tb + t_a); tdry.b = reinterpret_cast<int32_t *>(tb + t_b);
     tdry.f = tb + t_f; tdry.g = tb + t_g; tdry.ok = tb + t_ok;
@@ -2184,7 +2258,15 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     if (soft) { soft_seq[k] = ++soft_next; soft_klass[k] = et.klass; }
     const double tl0 = now_ms();
     const unsigned grid = (unsigned)((N * 16 + 255) / 256);
-    if (soft) {
+    if (guard_on) {  // sessions where pdb or cdp votes: the GUARD instances
+      if (soft) {
+        if (R <= 8) k_evict_rank<16, 8, true, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
+        else k_evict_rank<16, VC_MAX_DIMS, true, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
+      } else {
+        if (R <= 8) k_evict_rank<16, 8, false, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
+        else k_evict_rank<16, VC_MAX_DIMS, false, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
+      }
+    } else if (soft) {
       if (R <= 8) k_evict_rank<16, 8, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
       else k_evict_rank<16, VC_MAX_DIMS, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
     } else {
@@ -2310,7 +2392,10 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
         if (rc2) return rc2;
         idx_live = 0;
       }
-      (samp ? k_evict_dryrun<true> : k_evict_dryrun<false>)<<<(unsigned)((N + 127) / 128), 128, 0, s->stream>>>(tv, tt, dr);
+      void (*const dry_fn)(vct::TopoView, vct::TopoTask, TopoDry) =
+          guard_on ? (samp ? k_evict_dryrun<true, true> : k_evict_dryrun<false, true>)
+                   : (samp ? k_evict_dryrun<true> : k_evict_dryrun<false>);
+      dry_fn<<<(unsigned)((N + 127) / 128), 128, 0, s->stream>>>(tv, tt, dr);
       (samp ? k_evict_select<true> : k_evict_select<false>)<<<1, 1024, 0, s->stream>>>(sel);
       launches += 2;
       CUDA_TRY(cudaGetLastError());

@@ -98,6 +98,8 @@ class Engine:
         _check(self.L.vc_snapshot_set_running(self.h, C.byref(rt) if rt is not None else None, tf))
         po = s.preempt_options()  # the preempt action's arguments; restated on every upload, None restores the defaults
         _check(self.L.vc_snapshot_set_preempt_options(self.h, C.byref(po) if po is not None else None))
+        vg = s.victim_guards()  # the pdb / cdp votes' table; restated on every upload, None clears it
+        _check(self.L.vc_snapshot_set_victim_guards(self.h, C.byref(vg) if vg is not None else None))
         nom = getattr(s, "t_nominated", None)  # Pod.Status.NominatedNodeName per pending task; restated on every upload
         has_nom = nom is not None and s.T and bool((nom >= 0).any())
         _check(self.L.vc_snapshot_set_nominated(self.h, nom.ctypes.data_as(C.POINTER(C.c_int32)) if has_nom else None))

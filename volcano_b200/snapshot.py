@@ -18,7 +18,7 @@ import numpy as np
 from . import abi
 from .api import (HyperNode, Node, Pod, PodGroup, Queue, TASK_PRIORITY_ANNOTATION, allocated_status, get_task_role,
                   get_task_status, pod_index_under_task, quantity_milli, quantity_value, Taint, Toleration,
-                  NodeSelectorRequirement, pod_critical, pod_preemptable)
+                  NodeSelectorRequirement, PodDisruptionBudget, pod_cooldown_until, pod_critical, pod_preemptable)
 
 
 # ---------------------------------------------------------------------------------------
@@ -417,6 +417,32 @@ class Snapshot:
             pa.max_candidate_nodes_absolute, self.preempt_seed & (2 ** 64 - 1), self.now_ns, n,
             _ptr(self.rt_pod_priority if n > 0 else None, _I32), _ptr(self.rt_start_ns if n > 0 else None, _I64))
 
+    def victim_guards(self) -> Optional[abi.vc_victim_guards]:
+        """The argument of vc_snapshot_set_victim_guards, or None when the session has no table (no pdb / cdp plugin)."""
+        if getattr(self, "g_pdb_off", None) is None:
+            return None
+        return abi.vc_victim_guards(self.RT, len(self.g_pdb_allowed), _ptr(self.g_pdb_allowed, _I32), _ptr(self.g_pdb_off, _I32),
+                                    _ptr(self.g_pdb, _I32), _ptr(self.g_flags, _U32), _ptr(self.g_until, _I64), self.now_ns)
+
+    def set_victim_guards(self, run_pods: Sequence[Pod], pdbs: Sequence[PodDisruptionBudget]) -> None:
+        """Encode what the pdb and cdp votes read, as the Go shim does: per running task the PDBs that count it (namespace,
+        matchLabels, DisruptedPods), whether it has labels, and the end of its cooldown protection."""
+        off, lst = [0], []
+        self.g_flags = np.zeros(len(run_pods), np.uint32)
+        self.g_until = np.full(len(run_pods), abi.VC_COOLDOWN_NONE, np.int64)
+        for r, p in enumerate(run_pods):
+            if not p.labels:
+                self.g_flags[r] |= abi.VC_GUARD_NO_LABELS
+            else:
+                lst += [i for i, b in enumerate(pdbs) if b.counts(p)]
+            off.append(len(lst))
+            until = pod_cooldown_until(p)
+            if until is not None:
+                self.g_until[r] = until
+        self.g_pdb_allowed = np.array([b.disruptions_allowed for b in pdbs], np.int32)
+        self.g_pdb_off = np.array(off, np.int32)
+        self.g_pdb = np.array(lst, np.int32)
+
     def set_running(self, n: int):
         """Allocate the node.Tasks table (vc_running_tasks) for n occupying tasks."""
         f8, i4, i8, u4 = np.float64, np.int32, np.int64, np.uint32
@@ -710,7 +736,8 @@ def encode_hypernodes(s: "Snapshot", hypernodes: Sequence[HyperNode], podgroups:
 
 def encode_cluster(nodes: Sequence[Node], pods: Sequence[Pod], podgroups: Sequence[PodGroup],
                    queues: Sequence[Queue], conf: SchedulerConf, tdm_zone_active: Optional[Dict[str, bool]] = None,
-                   hypernodes: Optional[Sequence[HyperNode]] = None) -> Snapshot:
+                   hypernodes: Optional[Sequence[HyperNode]] = None,
+                   pdbs: Optional[Sequence[PodDisruptionBudget]] = None) -> Snapshot:
     # ---- dimensions: cpu, memory, then scalars sorted by name -------------------------------
     scalars = set()
     for n in nodes:
@@ -1079,6 +1106,9 @@ def encode_cluster(nodes: Sequence[Node], pods: Sequence[Pod], podgroups: Sequen
     if conf.configurations.get("preempt"):
         s.preempt_args = preempt_arguments(conf)
         s.preempt_seed, s.now_ns = conf.preempt_seed, conf.now_ns
+    if any(p.name in ("pdb", "cdp") for tier in conf.tiers for p in tier):
+        s.now_ns = conf.now_ns
+        s.set_victim_guards(run_pods, pdbs or ())
     if hypernodes is not None:
         encode_hypernodes(s, hypernodes, podgroups, job_pods)
     if any(p.hierarchy for tier in conf.tiers for p in tier if p.name == "drf"):

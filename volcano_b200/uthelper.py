@@ -16,7 +16,7 @@ from typing import Callable, Dict, List, Optional, Sequence
 import numpy as np
 
 from . import abi
-from .api import BuildQueueWithAnnos, HyperNode, Node, Pod, PodGroup, Queue  # noqa: F401  (util.BuildQueueWithAnnos)
+from .api import BuildQueueWithAnnos, HyperNode, Node, Pod, PodDisruptionBudget, PodGroup, Queue  # noqa: F401  (util.BuildQueueWithAnnos)
 from .snapshot import PluginOption, SchedulerConf, Snapshot, encode_cluster
 
 
@@ -48,13 +48,14 @@ class TestCommonStruct:
     ExpectEvictNum: Optional[int] = None
     TdmZoneActive: Optional[Dict[str, bool]] = None
     HyperNodes: Optional[List[HyperNode]] = None  # HyperNodesMap of the reference harness
+    PDBs: Optional[List[PodDisruptionBudget]] = None  # what the pdb plugin lists through the informer factory
 
     def RegisterSession(self, tiers: Sequence[Sequence[PluginOption]], actions=("allocate",), **conf_kw) -> Snapshot:
         """conf_kw: fields of SchedulerConf, e.g. configurations={"preempt": {...}} for the reference's
         RegisterSession(tiers, []conf.Configuration)."""
         self.conf = SchedulerConf(tiers=[list(t) for t in tiers], actions=tuple(actions), **conf_kw)
         self.snap = encode_cluster(self.Nodes, self.Pods, self.PodGroups, self.Queues, self.conf,
-                                   tdm_zone_active=self.TdmZoneActive, hypernodes=self.HyperNodes)
+                                   tdm_zone_active=self.TdmZoneActive, hypernodes=self.HyperNodes, pdbs=self.PDBs)
         return self.snap
 
     def Run(self, engine) -> AllocateResult:
