@@ -578,7 +578,8 @@ func (a *followUp) Execute(ssn *framework.Session) {
 		rc = C.vc_reclaim_run(cur.snap, &res)
 	}
 	if rc != 0 {
-		fail(a.name) // VC_EUNSUPPORTED: the configuration is outside the path and nothing was applied; the session state is
+		fail(a.name) // VC_EUNSUPPORTED (tdm, BestEffort preemptors, ...): the configuration is outside the path and nothing
+		// was applied (network-topology-aware sessions and soft-mode topology jobs run on the library); the session state is
 		// what the earlier replays left, so the reference's action can take over from here
 		runStock(a.name, ssn)
 		return

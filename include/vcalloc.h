@@ -572,8 +572,18 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out);
    PreferNoSchedule taints under TaintToleration's batch score order preempt's normal reading: the count of intolerable
    ones is normalised by its maximum over predicateNodes (every node passing the static predicate, or under sampling the
    sampled list), candidates or not; reclaim and the topology-aware reading do not score nodes.
-   VC_EUNSUPPORTED: BestEffort pending tasks in the session (vc_snapshot_set_backfill), jobs with a network topology,
-   the tdm / network-topology-aware plugins; under sampling, enablePredicateErrorCache with a job
+   network-topology-aware (hypernode binpacking of normal pods, hypernode.binpack.normal-pod.enable): preempt's normal
+   reading adds the plugin's node score to util.PrioritizeNodes' total (batchNodeOrderFnForNormalPods + scaleFinalScore,
+   network_topology_aware.go:461-498), read from hyperNodeResourceCache.used as the session stands: the opening rows,
+   then allocate's kept operations in order, then every Statement Evict (-Resreq), Pipeline (+Resreq) and Discard (the
+   inverse, in reverse order) of preempt and reclaim, on every hypernode that holds the node, cpu, memory and the
+   task's present scalars. The sums are exact for integer-valued requests (the node rows follow the same rule). A node's
+   hypernode at a tier is the one of vc_hypernodes.member (where hypernodes of one tier overlap, the reference breaks out
+   of a Go map walk; the encoder keeps the lowest name); node.Tasks are walked in ascending running-task index. Jobs with
+   a (soft-mode) network topology never preempt, in either phase or reading (preempt.go:132-137); they reclaim, and their
+   pods are victims like any other. Reclaim and the topology-aware reading do not score nodes.
+   VC_EUNSUPPORTED: BestEffort pending tasks in the session (vc_snapshot_set_backfill), the tdm plugin; under sampling,
+   enablePredicateErrorCache with a job
    whose named roles span several (class, request) groups, and min_nodes_to_find below 1 (numNodesToFind of a list can
    then be 0; a session whose numNodesToFind(N) is 0 is refused too, although allocate runs it without sampling). */
 int vc_preempt_run(vc_snapshot *s, vc_result **out);

@@ -267,6 +267,60 @@ def make_guard_case(seed):
     return tc, tiers, actions, conf
 
 
+def make_nta_case(seed):
+    """The network-topology-aware plugin: the clusters of make_guard_case (pdb / cdp, the topology-aware reading, sampling),
+    make_soft_case (PreferNoSchedule taints) or make_samp_case, widened to at least 4 nodes, under a HyperNode tree of
+    1- to 4-node leaves (tier 1; some nodes in no leaf), two tier-2 halves and, often, a tier-3 root; a third of the jobs,
+    running or pending, in soft network-topology mode; the plugin in a random tier with random weights, fading 0 / 0.5
+    / 0.8, and hypernode binpacking of normal pods on in most cases. -> (TestCommonStruct, tiers, actions, conf)."""
+    from volcano_b200.api import BuildHyperNode
+    rnd = random.Random(seed * 104651 + 17)
+    family = rnd.random()
+    if family < 0.4:
+        tc, tiers, actions, conf = make_guard_case(seed)
+    elif family < 0.7:
+        tc, tiers, actions, conf = make_soft_case(seed)
+    else:
+        tc, tiers, actions, conf = make_samp_case(seed)
+    for i in range(len(tc.Nodes), 4):
+        tc.Nodes.append(BuildNode(f"n{i}", BuildResourceList(str(rnd.choice([2, 3, 4])), rnd.choice(["4G", "8G", "16G"]),
+                                                               ("pods", str(rnd.choice([3, 6, 20]))))))
+    names = [n.name for n in tc.Nodes]
+    rnd.shuffle(names)
+    leaves, i = [], 0
+    while i < len(names):
+        k = rnd.randint(1, 4)
+        if rnd.random() < 0.85:  # the other nodes belong to no leaf: FullScore on tier 1
+            leaves.append(BuildHyperNode(f"leaf{len(leaves)}", 1, [(m, "Node") for m in names[i:i + k]]))
+        i += k
+    hypernodes = list(leaves)
+    if len(leaves) >= 2 and rnd.random() < 0.8:
+        half = len(leaves) // 2
+        hypernodes.append(BuildHyperNode("midA", 2, [(h.name, "HyperNode") for h in leaves[:half]]))
+        hypernodes.append(BuildHyperNode("midB", 2, [(h.name, "HyperNode") for h in leaves[half:]]))
+        if rnd.random() < 0.6:
+            hypernodes.append(BuildHyperNode("root", 3, [("midA", "HyperNode"), ("midB", "HyperNode")]))
+    tc.HyperNodes = hypernodes
+    for pg in tc.PodGroups:
+        if rnd.random() < 0.33:
+            pg.network_topology_mode = "soft"
+            pg.__post_init__()
+    args = {"weight": rnd.choice([1, 10]), "hypernode.binpack.cpu": rnd.choice([1, 5]),
+            "hypernode.binpack.memory": rnd.choice([0, 1, 2]),
+            "hypernode.binpack.normal-pod.enable": rnd.random() < 0.85,
+            "hypernode.binpack.normal-pod.fading": rnd.choice([0, 0.5, 0.8])}
+    t = rnd.randrange(len(tiers))
+    tiers[t].insert(rnd.randint(0, len(tiers[t])), PluginOption.defaults("network-topology-aware", args))
+    if not any(a in ("preempt", "reclaim") for a in actions):
+        actions = actions + ("preempt",)
+    return tc, tiers, actions, conf
+
+
+def without_nta(tiers):
+    """The tiers without the network-topology-aware plugin."""
+    return [[o for o in t if o.name != "network-topology-aware"] for t in tiers if any(o.name != "network-topology-aware" for o in t)]
+
+
 def _plugins_and_actions(rnd):
     voters = [n for n in ("conformance", "gang", "priority", "drf", "proportion") if rnd.random() < 0.75]
     scorers = [n for n in ("predicates", "nodeorder", "binpack") if rnd.random() < 0.5]

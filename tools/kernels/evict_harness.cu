@@ -144,7 +144,30 @@ struct EhSoftArgs {
   unsigned long long *word;       // the reduction word after the launches
 };
 
-static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx, const uint8_t *guard = nullptr);
+// network-topology-aware's hypernode binpacking (the NTA instances): the plugin's tables as vcalloc.cu stages them.
+// member [L][N] (-1: the node is in no hypernode of that tier level), hn_alloc / hn_used [R][H], the tier weights [L]
+// (their total is summed here in level order, as the library does), the plugin's weight and per-dimension weights [R]
+// (-1: not weighed). nta_term [N] receives the per-node term the SOFT+NTA ranking stores (0 where it stores none).
+struct EhNtaArgs {
+  int L, H, weight;
+  const int32_t *member;
+  const double *hn_alloc, *hn_used, *tier_w;
+  const int32_t *dim_weight;
+  double *nta_term;
+};
+
+static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx, const uint8_t *guard = nullptr, const EhNtaArgs *nx = nullptr);
+
+static bool nta_check(const EhNtaArgs *x, int N, int R) {
+  if (!x || x->L < 1 || x->L > VC_MAX_TIERS || x->H < 1 || !x->member || !x->hn_alloc || !x->hn_used || !x->tier_w ||
+      !x->dim_weight || !x->nta_term)
+    return false;
+  for (size_t i = 0; i < (size_t)x->L * N; ++i)
+    if (x->member[i] < -1 || x->member[i] >= x->H) return false;
+  for (int d = 0; d < R; ++d)
+    if (x->dim_weight[d] < -1) return false;
+  return true;
+}
 
 extern "C" int eh_rank(const EhRankArgs *a) { return rank_run(a, nullptr); }
 
@@ -164,7 +187,25 @@ extern "C" int eh_soft_chain(const EhRankArgs *a, const EhSoftArgs *sx) {
   return rank_run(a, sx);
 }
 
+// The NTA instance k_evict_rank<16, .., false, false, true> of preempt's normal reading: cand / key as eh_rank, the key
+// carrying the plugin's term (the node-order plugins stay off, so the total is 0.0 + (0.0 + term))
+extern "C" int eh_nta_rank(const EhRankArgs *a, const EhNtaArgs *x) {
+  if (!a || a->mode == EV_MODE_RECLAIM || !nta_check(x, a->N, a->R)) return EH_EINVAL;
+  return rank_run(a, nullptr, nullptr, x);
+}
+
+// The SOFT+NTA chain: k_evict_rank<.., true, false, true> (the term goes to nta_term), k_evict_samp<true> under sampling,
+// then k_evict_pick / k_evict_pick_big <SAMP, true, true> until the candidates run out
+extern "C" int eh_nta_soft_chain(const EhRankArgs *a, const EhSoftArgs *sx, const EhNtaArgs *x) {
+  if (!a || !nta_check(x, a->N, a->R)) return EH_EINVAL;
+  if (!sx || !sx->order || !sx->n_order || !sx->word || a->N < 1 || a->mode == EV_MODE_RECLAIM) return EH_EINVAL;
+  if ((sx->samp != 0 && sx->samp != 1) || (sx->big != 0 && sx->big != 1) || sx->start < 0) return EH_EINVAL;
+  if (!sx->big && a->N > eh_pick_smem_max_nodes()) return EH_EINVAL;
+  return rank_run(a, sx, nullptr, x);
+}
+
 // p / t as rank_run built them (device rows staged, cand / key allocated); rank_run's buffers outlive the call
+template <bool NTA>
 static int soft_chain(const EhRankArgs *a, const EhSoftArgs &sx, EvictParams p, const EvictTask &t) {
   const int N = a->N;
   p.c.batch_any = 1; p.c.taint_batch = 1; p.c.w_taint = sx.w_taint;
@@ -176,8 +217,7 @@ static int soft_chain(const EhRankArgs *a, const EhSoftArgs &sx, EvictParams p, 
   EH_TRY(words.put(w0, 2));
   p.soft_word = word.d; p.soft_seq = sx.seq; p.soft_klass = 0; p.soft_reduce = sx.samp ? 0 : 1;
   p.samp_list = list.d; p.samp_cnt = words.d;
-  if (a->R <= 8) k_evict_rank<16, 8, true><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);
-  else k_evict_rank<16, VC_MAX_DIMS, true><<<(unsigned)(((size_t)N * 16 + 255) / 256), 256>>>(p, t);
+  launch_evict_rank<true, false, NTA>((unsigned)(((size_t)N * 16 + 255) / 256), 0, (size_t)a->R, p, t);
   EH_TRY(cudaGetLastError());
   if (sx.samp) {
     EvictSamp s;
@@ -192,8 +232,8 @@ static int soft_chain(const EhRankArgs *a, const EhSoftArgs &sx, EvictParams p, 
   EH_TRY(pick.alloc(EV_PICK_K + 1));
   p.pick_node = pick.d;
   const size_t smem = (size_t)N * 8;
-  auto fn = sx.samp ? k_evict_pick<true, true> : k_evict_pick<false, true>;
-  auto fn_big = sx.samp ? k_evict_pick_big<true, true> : k_evict_pick_big<false, true>;
+  auto fn = sx.samp ? k_evict_pick<true, true, NTA> : k_evict_pick<false, true, NTA>;
+  auto fn_big = sx.samp ? k_evict_pick_big<true, true, NTA> : k_evict_pick_big<false, true, NTA>;
   if (!sx.big && smem > 48 * 1024) EH_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int n_out = 0;
   for (int seq = 1;; ++seq) {  // as the host control loop drains a ranking: until a batch comes back short
@@ -216,7 +256,7 @@ static int soft_chain(const EhRankArgs *a, const EhSoftArgs &sx, EvictParams p, 
   return EH_OK;
 }
 
-static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx, const uint8_t *guard) {
+static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx, const uint8_t *guard, const EhNtaArgs *nx) {
   if (!a) return EH_EINVAL;
   const int N = a->N, R = a->R, RT = a->RT, J = a->J, Q = a->Q;
   if (N < 0 || R < 2 || R > VC_MAX_DIMS || RT < 0 || J < 0 || Q < 0 || a->pods_dim < -1 || a->pods_dim >= R) return EH_EINVAL;
@@ -282,10 +322,27 @@ static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx, const uint8_t *gu
   t.qalloc_has = a->qalloc_has; t.qdes_has = a->qdes_has;
   if (a->quota_on)
     for (int d = 0; d < R; ++d) { t.qalloc[d] = a->qalloc[d]; t.qdes[d] = a->qdes[d]; }
-  if (sx) return soft_chain(a, *sx, p, t);
+  DevBuf<int32_t> hn_member;
+  DevBuf<double> hn_alloc, hn_used, nta_term;
+  if (nx) {  // DevConf's plugin fields as vcalloc.cu derives them for nta_on
+    EH_TRY(hn_member.put(nx->member, (size_t)nx->L * N)); EH_TRY(hn_alloc.put(nx->hn_alloc, (size_t)R * nx->H));
+    EH_TRY(hn_used.put(nx->hn_used, (size_t)R * nx->H)); EH_TRY(nta_term.put(nullptr, N));
+    p.c.batch_any = 1; p.c.nta_plugin = 1; p.c.nta_tables = 1; p.c.nta_on = 1; p.c.nta_weight = nx->weight;
+    p.c.nta_L = nx->L; p.c.tier_w_total = 0.0;
+    for (int l = 0; l < nx->L; ++l) { p.c.tier_w[l] = nx->tier_w[l]; p.c.tier_w_total += nx->tier_w[l]; }
+    for (int d = 0; d < VC_MAX_DIMS; ++d) p.c.nta_dim_weight[d] = d < R ? nx->dim_weight[d] : -1;
+    p.hn_H = nx->H; p.hn_member = hn_member.d; p.hn_alloc = hn_alloc.d; p.hn_used = hn_used.d; p.nta_term = nta_term.d;
+  }
+  if (sx) {
+    const int rc = nx ? soft_chain<true>(a, *sx, p, t) : soft_chain<false>(a, *sx, p, t);
+    if (rc == EH_OK && nx) EH_TRY(nta_term.get(nx->nta_term, N));
+    return rc;
+  }
   if (N > 0) {  // the instance vcalloc.cu picks for R
     const unsigned grid = (unsigned)(((size_t)N * 16 + 255) / 256);
-    if (guard) {
+    if (nx) {
+      launch_evict_rank<false, false, true>(grid, 0, (size_t)R, p, t);
+    } else if (guard) {
       if (R <= 8) k_evict_rank<16, 8, false, true><<<grid, 256>>>(p, t);
       else k_evict_rank<16, VC_MAX_DIMS, false, true><<<grid, 256>>>(p, t);
     } else {
@@ -297,6 +354,7 @@ static int rank_run(const EhRankArgs *a, const EhSoftArgs *sx, const uint8_t *gu
   EH_TRY(cudaDeviceSynchronize());
   EH_TRY(cand.get(a->cand, N));
   EH_TRY(key.get(a->key, N));
+  if (nx) EH_TRY(nta_term.get(nx->nta_term, N));
   return EH_OK;
 }
 
@@ -315,7 +373,31 @@ struct EhApplyArgs {
   int undo;
 };
 
-extern "C" int eh_apply(const EhApplyArgs *a) {
+// The NTA instance k_evict_apply<true>: hyperNodeResourceCache.used [R][H] booked on every tier level's hypernode of the
+// node (member [L][N]), for dims 0, 1 and the present scalars (rt_has [RT] per victim, has for the preemptor); updated in
+// place.
+struct EhNtaApply {
+  int L, H;
+  const int32_t *member;
+  double *hn_used;
+  const uint32_t *rt_has;
+  uint32_t has;
+};
+
+static int apply_run(const EhApplyArgs *a, const EhNtaApply *x);
+
+extern "C" int eh_apply(const EhApplyArgs *a) { return apply_run(a, nullptr); }
+
+extern "C" int eh_apply_nta(const EhApplyArgs *a, const EhNtaApply *x) {
+  if (!a || !x || x->L < 1 || x->L > VC_MAX_TIERS || x->H < 1 || !x->member || !x->hn_used || (a->RT > 0 && !x->rt_has))
+    return EH_EINVAL;
+  if (a->N < 1) return EH_EINVAL;
+  for (size_t i = 0; i < (size_t)x->L * a->N; ++i)
+    if (x->member[i] < -1 || x->member[i] >= x->H) return EH_EINVAL;
+  return apply_run(a, x);
+}
+
+static int apply_run(const EhApplyArgs *a, const EhNtaApply *x) {
   if (!a) return EH_EINVAL;
   const int N = a->N, R = a->R, K = a->K, RT = a->RT;
   if (N < 1 || R < 1 || R > VC_MAX_DIMS || K < 0 || K > VC_MAX_KDIMS || RT < 0) return EH_EINVAL;
@@ -348,9 +430,21 @@ extern "C" int eh_apply(const EhApplyArgs *a) {
   for (int d = 0; d < R; ++d) t.rec.req[d] = a->req[d];
   for (int k = 0; k < K; ++k) t.rec.kreq[k] = a->kreq_t[k];
   for (int k = 0; k < 2; ++k) t.rec.knz[k] = a->knz_t[k];
-  k_evict_apply<<<1, 64>>>(p, t, a->undo ? 1 : 0);
+  DevBuf<int32_t> hn_member;
+  DevBuf<double> hn_used;
+  DevBuf<uint32_t> rt_has;
+  if (x) {
+    EH_TRY(hn_member.put(x->member, (size_t)x->L * N)); EH_TRY(hn_used.put(x->hn_used, (size_t)R * x->H));
+    EH_TRY(rt_has.put(x->rt_has, RT));
+    p.c.nta_L = x->L; p.hn_H = x->H; p.hn_member = hn_member.d; p.hn_used = hn_used.d; p.rt_has = rt_has.d;
+    t.rec.has = x->has;
+    k_evict_apply<true><<<1, 64>>>(p, t, a->undo ? 1 : 0);
+  } else {
+    k_evict_apply<<<1, 64>>>(p, t, a->undo ? 1 : 0);
+  }
   EH_TRY(cudaGetLastError());
   EH_TRY(cudaDeviceSynchronize());
+  if (x) EH_TRY(hn_used.get(x->hn_used, (size_t)R * x->H));
   EH_TRY(rel.get(a->rel, (size_t)R * N)); EH_TRY(pip.get(a->pip, (size_t)R * N)); EH_TRY(kreq.get(a->kreq, (size_t)K * N));
   EH_TRY(knz.get(a->knz, (size_t)2 * N)); EH_TRY(pod_count.get(a->pod_count, N)); EH_TRY(rt_ev.get(a->rt_evicted, RT));
   return EH_OK;

@@ -76,6 +76,16 @@ struct EvictParams {
   int soft_klass, soft_reduce;
   // GUARD instances (pdb or cdp votes in the action): vct::VCT_GUARD_* bits per running task
   const uint8_t *rt_guard;
+  // network-topology-aware with hypernode binpacking of normal pods (DevConf::nta_on): hn_used is the evicting actions'
+  // working copy of hyperNodeResourceCache.used, which k_evict_apply books in every action; the NTA instances of
+  // k_evict_rank add the plugin's node score to preempt's key. SOFT+NTA: the ranking stores the score per node in
+  // nta_term (one array per ranking set) and the pick adds it when it finishes total_score.
+  int hn_H;
+  const int32_t *hn_member;  // [L][N] hypernode of the node at each tier level, -1 none
+  const double *hn_alloc;    // [R][H]
+  double *hn_used;           // [R][H]
+  const uint32_t *rt_has;    // [RT] resource presence bits of the running tasks (the events book dims 0, 1 and these)
+  double *nta_term;          // [N]
 };
 
 struct EvNodeView {
@@ -102,12 +112,26 @@ __device__ __forceinline__ int ev_max_soft(const EvictParams &p) {
   return (w >> 8) == p.soft_seq ? (int)(w & 0xffull) : 0;
 }
 // the pick's order key of a node: SOFT adds TaintToleration's normalised score to the stored order part, in total_score's
-// operation order (0.0 + order, then + batch: the same double as a single call on the node)
-template <bool SOFT>
+// operation order (0.0 + order, then + batch: the same double as a single call on the node); NTA adds the stored
+// network-topology-aware term as the batch's second addend
+template <bool SOFT, bool NTA = false>
 __device__ __forceinline__ unsigned long long ev_pick_key(const EvictParams &p, int node, int max_soft) {
   if (!SOFT) return p.key[node];
   const int soft = (int)((p.cstat[(size_t)p.soft_klass * p.d.N + node] >> CS_SOFT_SHIFT) & 0xffu);
-  return ev_score_key(total_score(p.c, true, __longlong_as_double((long long)p.key[node]), soft, max_soft));
+  return ev_score_key(total_score(p.c, true, __longlong_as_double((long long)p.key[node]), soft, max_soft,
+                                  NTA ? p.nta_term[node] : 0.0));
+}
+
+// batchNodeOrderFnForNormalPods + scaleFinalScore (network_topology_aware.go:461-498, :758-764) for node n, on the working
+// copy of hyperNodeResourceCache: the same function allocate's dense pass calls (nta_node_score)
+__device__ __forceinline__ double ev_nta_score(const EvictParams &p, const TaskRec &t, int n) {
+  const int H = p.hn_H;
+  return nta_node_score(p.c, [&](int l) {
+    const int h = p.hn_member[(size_t)l * p.d.N + n];
+    return h < 0 ? 1.0
+                 : hn_binpack_score(p.c, p.d.R, t, [&](int d) { return p.hn_used[(size_t)d * H + h]; },
+                                    [&](int d) { return p.hn_alloc[(size_t)d * H + h]; });
+  });
 }
 
 // the action's candidate filter on one task of node.Tasks
@@ -170,7 +194,8 @@ __device__ __forceinline__ bool ev_may_be_victim(const EvictParams &p, const Evi
 // SOFT: the key is the order part only, and with soft_reduce every node passing the static predicate (candidate or not:
 // predicateNodes, scheduler_helper.go:76-136) enters the soft-taint maximum, one warp max and at most one atomic per warp.
 // GUARD: the pdb and cdp votes take part in ev_may_be_victim.
-template <int LPN, int RMAX, bool SOFT = false, bool GUARD = false>
+// NTA: network-topology-aware's node score enters preempt's key (SOFT: it goes to nta_term, the pick adds it).
+template <int LPN, int RMAX, bool SOFT = false, bool GUARD = false, bool NTA = false>
 __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) {
   const size_t gid = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   const int n = (int)(gid / LPN);
@@ -246,13 +271,22 @@ __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) 
         const EvNodeView nv{p, n};
         double order = 0.0;
         const bool has_order = node_order(p.c, R, K, t.rec, nv, cs, &order);
+        const double nta = NTA ? ev_nta_score(p, t.rec, n) : 0.0;
         if (SOFT) key = (unsigned long long)__double_as_longlong(has_order ? order : 0.0);
-        else key = ev_score_key(total_score(p.c, has_order, has_order ? order : 0.0, 0, 0));
+        else key = ev_score_key(total_score(p.c, has_order, has_order ? order : 0.0, 0, 0, nta));
+        if (SOFT && NTA) p.nta_term[n] = nta;
       }
     }
   }
   p.cand[n] = cand;
   p.key[n] = key;
+}
+
+// k_evict_rank with 16 lanes per node, for R <= 8 or up to VC_MAX_DIMS resource dimensions
+template <bool SOFT, bool GUARD, bool NTA>
+inline void launch_evict_rank(unsigned grid, cudaStream_t st, size_t R, const EvictParams &p, const EvictTask &t) {
+  if (R <= 8) k_evict_rank<16, 8, SOFT, GUARD, NTA><<<grid, 256, 0, st>>>(p, t);
+  else k_evict_rank<16, VC_MAX_DIMS, SOFT, GUARD, NTA><<<grid, 256, 0, st>>>(p, t);
 }
 
 // one block: the next EV_PICK_K candidates in the action's node order (preempt: score descending, lowest index first
@@ -263,7 +297,7 @@ __global__ void __launch_bounds__(256) k_evict_rank(EvictParams p, EvictTask t) 
 // memory (k_evict_pick below): repairs read the candidate flags and keys from global memory.
 // The last store of the launch is `seq` into pick_node[EV_PICK_K] (system scope): the host polls that word of the mapped
 // buffer instead of paying a stream synchronisation per hand-out. SOFT: the keys are finished here (ev_pick_key).
-template <bool SAMP, bool SOFT = false>
+template <bool SAMP, bool SOFT = false, bool NTA = false>
 __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
   __shared__ unsigned long long s_key[32];
   __shared__ int s_node[32];
@@ -284,7 +318,7 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
     bk = 0ull; bn = -1;
     for (int n = threadIdx.x; n < N; n += blockDim.x) {
       if (n == skip || p.cand[node_of(n)] != 1) continue;
-      const unsigned long long k = mode == EV_MODE_RECLAIM ? 0ull : ev_pick_key<SOFT>(p, node_of(n), max_soft);
+      const unsigned long long k = mode == EV_MODE_RECLAIM ? 0ull : ev_pick_key<SOFT, NTA>(p, node_of(n), max_soft);
       if (bn < 0 || k > bk) { bk = k; bn = n; }  // ascending n per thread: the first of equal keys stays
     }
   };
@@ -343,7 +377,7 @@ __global__ void k_evict_pick_big(EvictParams p, int mode, int seq) {
 // EV_PICK_K candidates in order. Phase 2, one warp: a 32-way merge of those sorted lists. Same order as the sequential
 // tournament: key descending, node ascending. SOFT: the keys are finished while they are staged (ev_pick_key).
 extern __shared__ unsigned long long ev_pick_cache[];
-template <bool SAMP, bool SOFT = false>
+template <bool SAMP, bool SOFT = false, bool NTA = false>
 __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, int seq) {
   __shared__ unsigned long long l_key[32][EV_PICK_K];
   __shared__ int l_node[32][EV_PICK_K];
@@ -353,7 +387,7 @@ __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, in
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int max_soft = SOFT ? ev_max_soft(p) : 0;
   for (int n = threadIdx.x; n < N; n += blockDim.x)  // key + 1 (never wraps: see ev_score_key), 0 = not a candidate
-    ev_pick_cache[n] = p.cand[node_of(n)] == 1 ? (mode == EV_MODE_RECLAIM ? 1ull : ev_pick_key<SOFT>(p, node_of(n), max_soft) + 1ull)
+    ev_pick_cache[n] = p.cand[node_of(n)] == 1 ? (mode == EV_MODE_RECLAIM ? 1ull : ev_pick_key<SOFT, NTA>(p, node_of(n), max_soft) + 1ull)
                                                : 0ull;
   if (threadIdx.x < EV_PICK_K) s_pick[threadIdx.x] = -1;
   __syncwarp();  // a lane only ever reads the entries it wrote
@@ -421,13 +455,27 @@ __global__ void __launch_bounds__(1024) k_evict_pick(EvictParams p, int mode, in
 // Statement.Pipeline of the preemptor (Pipelined += Resreq; predicates AllocateFunc: AddPod) on node cmd[0]
 // `undo` != 0: the inverse in Statement.Discard's order (UnPipeline, then unevict the victims in reverse order), so that
 // with non-integer requests the rows come back exactly as the reference's discard leaves them.
+// With hn_used (nta_on), network-topology-aware's AllocateFunc / DeallocateFunc (network_topology_aware.go:309-340) book
+// the request on the hypernode of every tier level that holds the node, dims 0, 1 and the task's present scalars, in
+// the same order of events; thread d owns dimension d of every hypernode. Only the NTA instance books them.
+template <bool NTA = false>
 __global__ void k_evict_apply(EvictParams p, EvictTask t, int undo) {
   const int n = p.cmd[0], nv = p.cmd[1];
   const int N = p.d.N, R = p.d.R, K = p.d.K;
   const int d = threadIdx.x;
   const double sg = undo ? -1.0 : 1.0;
+  auto hn_book = [&](double v, uint32_t has) {
+    if constexpr (NTA) {
+      if (d >= 2 && !(has & (1u << d))) return;
+      for (int l = 0; l < p.c.nta_L; ++l) {
+        const int h = p.hn_member[(size_t)l * N + n];
+        if (h >= 0) p.hn_used[(size_t)d * p.hn_H + h] += v;
+      }
+    }
+  };
   auto pipeline = [&]() {
     if (d < R) p.pip[(size_t)d * N + n] += sg * t.rec.req[d];
+    if (NTA && d < R) hn_book(sg * t.rec.req[d], t.rec.has);
     if (p.c.has_predicates) {
       if (d >= 32 && d < 32 + K) p.kreq[(size_t)(d - 32) * N + n] += sg * t.rec.kreq[d - 32];
       if (d >= 48 && d < 50) p.knz[(size_t)(d - 48) * N + n] += sg * t.rec.knz[d - 48];
@@ -438,6 +486,7 @@ __global__ void k_evict_apply(EvictParams p, EvictTask t, int undo) {
   for (int i = 0; i < nv; ++i) {
     const int r = p.cmd[2 + (undo ? nv - 1 - i : i)];
     if (d < R) p.rel[(size_t)d * N + n] += sg * p.rt_req[(size_t)d * p.RT + r];
+    if (NTA && d < R) hn_book(-sg * p.rt_req[(size_t)d * p.RT + r], p.rt_has[r]);
     if (p.c.has_predicates) {
       if (d >= 32 && d < 32 + K) p.kreq[(size_t)(d - 32) * N + n] -= sg * p.rt_kreq[(size_t)(d - 32) * p.RT + r];
       if (d >= 48 && d < 50) p.knz[(size_t)(d - 48) * N + n] -= sg * p.rt_knz[(size_t)(d - 48) * p.RT + r];

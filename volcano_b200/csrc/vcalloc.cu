@@ -1915,10 +1915,8 @@ int ensure_evict_session(vc_snapshot *s) {
   if (s->dc.to_find > 0 && s->dc.enable_ecache && !s->all_pure)
     return fail(VC_EUNSUPPORTED, "preempt / reclaim under feasible-node sampling: enablePredicateErrorCache with a job whose "
                                  "named roles span several (class, request) groups (the role-keyed cache is not modelled)");
-  if (s->dc.nta_plugin || vch::has_plugin(s->conf, VC_PLUGIN_TDM))
-    return fail(VC_EUNSUPPORTED, "preempt / reclaim: the network-topology-aware and tdm plugins are outside the path");
-  for (uint8_t f : s->h_job_soft)
-    if (f) return fail(VC_EUNSUPPORTED, "preempt / reclaim: jobs with a network topology (preempt.go:131-135)");
+  if (vch::has_plugin(s->conf, VC_PLUGIN_TDM))
+    return fail(VC_EUNSUPPORTED, "preempt / reclaim: the tdm plugin is outside the path");
   if (s->es_built) return VC_OK;
   vch::EvictSession &e = s->es;
   e = vch::EvictSession();
@@ -1937,6 +1935,16 @@ int ensure_evict_session(vc_snapshot *s) {
   e.phase_flipped = s->alloc_ran && !s->conf.enqueue_action_enabled;
   if (s->dc.has_drf)
     for (size_t j = 0; j < J; ++j) e.drf_share((int)j);
+  // network-topology-aware's hyperNodeResourceCache.used: the opening rows plus allocate's AllocateFunc events (allocate's
+  // own copies are per-CTA replicas), booked in the order of the kept operations like the node rows below
+  const bool nta = s->dc.nta_on;
+  const size_t H = (size_t)s->hn_H, L = (size_t)s->hn_L;
+  std::vector<double> hn_used;
+  if (nta) {
+    hn_used.resize(R * H);
+    CUDA_TRY(cudaMemcpyAsync(hn_used.data(), s->hn_used0.d(s->in), R * H * 8, cudaMemcpyDeviceToHost, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));
+  }
   // Statement.Allocate / Pipeline of every kept visit of the allocate action, in order
   std::vector<double> &idle = e.n_idle;  // the host mirror of Idle moves with allocate's placements
   for (const vc_decision &op : s->last_dec) {
@@ -1949,6 +1957,12 @@ int ensure_evict_session(vc_snapshot *s) {
       for (size_t d = 0; d < R; ++d) e.n_pip[d * N + n] += k.t_req[d * T + t];
     }
     e.on_allocate(j, e.task_res(t), k.t_req.data(), (int)T, t);
+    for (size_t l = 0; nta && l < L; ++l) {
+      const int h = s->has_topo ? s->h_member[l * N + n] : 0;
+      if (h < 0) continue;
+      for (size_t d = 0; d < R; ++d)
+        if (d < 2 || (k.t_has[t] & (1u << d))) hn_used[d * H + h] += k.t_req[d * T + t];
+    }
   }
   s->last_dec.clear();  // applied (a second evicting action continues from e)
   s->t_filtered = vch::fit_error_node_kinds(s->last_fit.data(), s->last_fit.size(), k.t_role.data(), k.r_flags.data(), T);
@@ -1979,7 +1993,11 @@ int ensure_evict_session(vc_snapshot *s) {
                o_cand = take(N), o_prio = take(B * 4), o_jready = take(std::max<size_t>(J, 1) * 4), o_qover = take(std::max<size_t>(Q, 1)),
                o_key2 = take(N * 8), o_cand2 = take(N),  // second ranking scratch: the preemptor ranked one ahead
                o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4),  // k_evict_samp: lists, counts, indexes
-               o_soft = take(2 * 8);  // soft-taint maximum per ranking set (EvictParams::soft_word)
+               o_soft = take(2 * 8),  // soft-taint maximum per ranking set (EvictParams::soft_word)
+               // network-topology-aware binpacking: hyperNodeResourceCache.used, the running tasks' presence bits, the
+               // plugin's node score per ranking set (sizes 0, so no room, without it)
+               o_hn = take(nta ? R * (size_t)s->hn_H * 8 : 0), o_has = take(nta ? B * 4 : 0), o_nta = take(nta ? N * 8 : 0),
+               o_nta2 = take(nta ? N * 8 : 0);
   if (off > s->d_ev_bytes) {
     if (s->d_ev) cudaFree(s->d_ev);
     s->d_ev = nullptr;
@@ -1987,9 +2005,13 @@ int ensure_evict_session(vc_snapshot *s) {
     s->d_ev_bytes = off;
   }
   if (!s->h_ev) CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&s->h_ev), (EV_CMD_OFF + 2 + EV_MAX_VICTIMS) * 4, cudaHostAllocMapped));
-  (void)o_key2; (void)o_cand2; (void)o_list; (void)o_list2; (void)o_samp; (void)o_soft;
+  (void)o_key2; (void)o_cand2; (void)o_list; (void)o_list2; (void)o_samp; (void)o_soft; (void)o_nta; (void)o_nta2;
   unsigned char *base = reinterpret_cast<unsigned char *>(s->d_ev);
   CUDA_TRY(cudaMemsetAsync(base, 0, off, s->stream));
+  if (nta) {
+    CUDA_TRY(cudaMemcpyAsync(base + o_hn, hn_used.data(), R * H * 8, cudaMemcpyHostToDevice, s->stream));
+    if (s->rt.n > 0) CUDA_TRY(cudaMemcpyAsync(base + o_has, s->rt.has.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
+  }
   if (s->rt.n > 0) {
     const vch::RunningTasks &b = s->rt;
     CUDA_TRY(cudaMemcpyAsync(base + o_off, b.off.data(), (N + 1) * 4, cudaMemcpyHostToDevice, s->stream));
@@ -2033,6 +2055,9 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   const vch::EvictKeep &k = s->ek;
   const size_t B = (size_t)std::max(s->rt.n, 1);
   e.g = guard_on ? &s->guards : nullptr;
+  // network-topology-aware with hypernode binpacking: every action books hyperNodeResourceCache.used (a reclaim can run
+  // before a preempt on the same session); only preempt's normal reading ranks with the plugin's score
+  const bool nta = s->dc.nta_on;
   // device parameter block (same slab layout as ensure_evict_session)
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
@@ -2041,7 +2066,11 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
                o_cand = take(N), o_prio = take(B * 4), o_jready = take(std::max<size_t>(J, 1) * 4), o_qover = take(std::max<size_t>(Q, 1)),
                o_key2 = take(N * 8), o_cand2 = take(N),  // second ranking scratch: the preemptor ranked one ahead
                o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4),  // k_evict_samp: lists, counts, indexes
-               o_soft = take(2 * 8);  // soft-taint maximum per ranking set (EvictParams::soft_word)
+               o_soft = take(2 * 8),  // soft-taint maximum per ranking set (EvictParams::soft_word)
+               // network-topology-aware binpacking: hyperNodeResourceCache.used, the running tasks' presence bits, the
+               // plugin's node score per ranking set (sizes 0, so no room, without it)
+               o_hn = take(nta ? R * (size_t)s->hn_H * 8 : 0), o_has = take(nta ? B * 4 : 0), o_nta = take(nta ? N * 8 : 0),
+               o_nta2 = take(nta ? N * 8 : 0);
   unsigned char *base = reinterpret_cast<unsigned char *>(s->d_ev);
   EvictParams p;
   std::memset(&p, 0, sizeof p);
@@ -2089,6 +2118,10 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     d_pdb_allowed = reinterpret_cast<const int32_t *>(gb + g_allowed);
   }
   p.rt_guard = d_rt_guard;
+  if (nta) {
+    p.hn_H = s->hn_H; p.hn_member = s->hn_member.d(s->in); p.hn_alloc = s->hn_alloc.d(s->in);
+    p.hn_used = reinterpret_cast<double *>(base + o_hn); p.rt_has = reinterpret_cast<const uint32_t *>(base + o_has);
+  }
   // topology-aware preemption: the dry run's inputs beyond the ranking's, its per-node results and scratch
   const bool topo_on = !reclaim && s->popt.topology_aware;
   vct::TopoView tv;
@@ -2220,17 +2253,24 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   int pick_buf[EV_PICK_K], pick_pos = EV_PICK_K, pick_n = 0;
   // the pick kernel stages the candidates' keys in shared memory when they fit (N * 8 bytes)
   size_t pick_smem = N * 8 <= 200 * 1024 ? N * 8 : 0;
-  void (*const pick_fn)(EvictParams, int, int) = samp ? (soft ? k_evict_pick<true, true> : k_evict_pick<true, false>)
-                                                      : (soft ? k_evict_pick<false, true> : k_evict_pick<false, false>);
-  void (*const pick_big_fn)(EvictParams, int, int) = samp ? (soft ? k_evict_pick_big<true, true> : k_evict_pick_big<true, false>)
-                                                          : (soft ? k_evict_pick_big<false, true> : k_evict_pick_big<false, false>);
+  // preempt's normal reading with network-topology-aware binpacking ranks on the NTA instances; with SOFT the pick adds
+  // the plugin's term the ranking stored (without SOFT the ranking's key is final and the pick is the plain one)
+  const bool nta_rank = nta && !reclaim && !topo_on;
+  void (*const pick_fn)(EvictParams, int, int) =
+      samp ? (soft ? (nta_rank ? k_evict_pick<true, true, true> : k_evict_pick<true, true>) : k_evict_pick<true, false>)
+           : (soft ? (nta_rank ? k_evict_pick<false, true, true> : k_evict_pick<false, true>) : k_evict_pick<false, false>);
+  void (*const pick_big_fn)(EvictParams, int, int) =
+      samp ? (soft ? (nta_rank ? k_evict_pick_big<true, true, true> : k_evict_pick_big<true, true>) : k_evict_pick_big<true, false>)
+           : (soft ? (nta_rank ? k_evict_pick_big<false, true, true> : k_evict_pick_big<false, true>)
+                   : k_evict_pick_big<false, false>);
   if (pick_smem > 48 * 1024)
     CUDA_TRY(cudaFuncSetAttribute(pick_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pick_smem));
   double t_launch = 0.0, t_sync = 0.0;  // host time inside kernel launches / waiting for a hand-out (vc_stats.prof_cycles, us)
   // Two ranking scratch sets (candidate flags, keys, hand-out slots): while the host walks the candidates of one
   // preemptor the device already ranks the one the control loop will most likely try next (rk.hint). Most preemptors fail,
   // and a failed one leaves the session untouched, so the ranking made ahead is still exact; any eviction / pipeline /
-  // discard in between (`epoch`) voids it.
+  // discard in between (`epoch`) voids it. That includes network-topology-aware's hyperNodeResourceCache.used, which
+  // only k_evict_apply moves: a ranking made ahead read the same hn_used as a ranking made now would.
   struct RankSet { unsigned long long *key; uint8_t *cand; int32_t *d_pick; volatile int32_t *h_pick; int seq; };
   RankSet sets[2] = {{reinterpret_cast<unsigned long long *>(base + o_key), base + o_cand, dev_h, s->h_ev, 0},
                      {reinterpret_cast<unsigned long long *>(base + o_key2), base + o_cand2, dev_h + (EV_PICK_K + 1),
@@ -2243,6 +2283,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     EvictParams q = p;
     q.key = sets[k].key; q.cand = sets[k].cand; q.pick_node = sets[k].d_pick; q.samp_list = d_list[k]; q.samp_cnt = d_samp + k;
     q.soft_word = d_soft + k; q.soft_seq = soft_seq[k]; q.soft_klass = soft_klass[k]; q.soft_reduce = samp ? 0 : 1;
+    if (nta) q.nta_term = reinterpret_cast<double *>(base + (k ? o_nta2 : o_nta));
     return q;
   };
   auto launch_pick = [&](int k, int mode) -> int {
@@ -2258,7 +2299,10 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     if (soft) { soft_seq[k] = ++soft_next; soft_klass[k] = et.klass; }
     const double tl0 = now_ms();
     const unsigned grid = (unsigned)((N * 16 + 255) / 256);
-    if (guard_on) {  // sessions where pdb or cdp votes: the GUARD instances
+    if (nta_rank) {  // network-topology-aware binpacking in preempt's normal reading: the NTA instances
+      if (guard_on) (soft ? launch_evict_rank<true, true, true> : launch_evict_rank<false, true, true>)(grid, s->stream, R, with_set(k), et);
+      else (soft ? launch_evict_rank<true, false, true> : launch_evict_rank<false, false, true>)(grid, s->stream, R, with_set(k), et);
+    } else if (guard_on) {  // sessions where pdb or cdp votes: the GUARD instances
       if (soft) {
         if (R <= 8) k_evict_rank<16, 8, true, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
         else k_evict_rank<16, VC_MAX_DIMS, true, true><<<grid, 256, 0, s->stream>>>(with_set(k), et);
@@ -2343,7 +2387,8 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     CUDA_TRY(cudaStreamSynchronize(s->stream));  // the previous command has been consumed
     h_cmd[0] = node; h_cmd[1] = (int32_t)victims.size();
     for (size_t i = 0; i < victims.size(); ++i) h_cmd[2 + i] = victims[i];
-    k_evict_apply<<<1, 64, 0, s->stream>>>(p, et, undo);
+    if (nta) k_evict_apply<true><<<1, 64, 0, s->stream>>>(p, et, undo);
+    else k_evict_apply<<<1, 64, 0, s->stream>>>(p, et, undo);
     launches++;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(s->stream));
@@ -2452,6 +2497,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
       if (job_pending((int)j) || !k.j_valid[j]) continue;
       const int q = k.j_queue[j];
       if (q < 0 || !e.job_starving((int)j)) continue;
+      if (!s->h_job_soft.empty() && s->h_job_soft[j]) continue;  // jobs with a network topology never preempt (preempt.go:132-137)
       has_q[q] = 1;
       preemptors[q].push((int)j);
       under_request[q].push_back((int)j);
