@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -110,16 +111,64 @@ double now_ms() {
   return duration<double, std::milli>(steady_clock::now().time_since_epoch()).count();
 }
 
-// One device arena + one pinned staging arena per snapshot: the whole session goes up in a single
-// cudaMemcpyAsync (SURVEY §8f-2 'upload once per cycle').
-struct Arena {
-  unsigned char *dev = nullptr, *pin = nullptr;
-  size_t cap = 0, used = 0;
-  size_t reserve(size_t bytes) {
-    size_t off = (used + 255) & ~(size_t)255;
+// One owned allocation of device memory, pinned host memory or pinned host memory mapped into the device's address
+// space. It only grows, keeps no contents across a reallocation and never zeroes anything; the snapshot's destructor
+// releases every one.
+enum class Mem { Device, Pinned, Mapped };
+template <class T, Mem M = Mem::Device>
+class Buf {
+ public:
+  Buf() = default;
+  Buf(const Buf &) = delete;
+  Buf &operator=(const Buf &) = delete;
+  ~Buf() { release(); }
+  int reserve(size_t bytes) {
+    bytes = std::max<size_t>(bytes, 16);
+    if (p_ && bytes <= cap_) return VC_OK;
+    release();
+    void *q = nullptr;
+    const cudaError_t e = M == Mem::Device ? cudaMalloc(&q, bytes)
+                          : M == Mem::Pinned ? cudaMallocHost(&q, bytes)
+                                             : cudaHostAlloc(&q, bytes, cudaHostAllocMapped);
+    if (e != cudaSuccess) {
+      cudaGetLastError();  // a non-sticky error must not fail the next call's check
+      return fail(VC_ECUDA, "allocating %zu bytes: %s", bytes, cudaGetErrorString(e));
+    }
+    p_ = static_cast<T *>(q);
+    cap_ = bytes;
+    return VC_OK;
+  }
+  size_t capacity() const { return cap_; }
+  operator T *() const { return p_; }
+
+ private:
+  void release() {
+    if (p_) (M == Mem::Device ? cudaFree(p_) : cudaFreeHost(p_));
+    p_ = nullptr;
+    cap_ = 0;
+  }
+  T *p_ = nullptr;
+  size_t cap_ = 0;
+};
+
+// The regions of one slab: each starts at the next multiple of 256 bytes after the previous one
+struct Layout {
+  size_t used = 0;
+  size_t take(size_t bytes) {
+    const size_t off = (used + 255) & ~(size_t)255;
     used = off + bytes;
     return off;
   }
+  size_t padded() const { return (used + 255) & ~(size_t)255; }
+};
+template <class T>
+T *at(unsigned char *base, size_t off) { return reinterpret_cast<T *>(base + off); }
+
+// One device arena + one pinned staging arena per snapshot: the whole session goes up in a single
+// cudaMemcpyAsync (SURVEY §8f-2 'upload once per cycle').
+struct Arena : Layout {
+  Buf<unsigned char> dev;
+  Buf<unsigned char, Mem::Pinned> pin;
 };
 
 template <class T>
@@ -179,12 +228,11 @@ struct vc_snapshot {
   Slot<int32_t> s_heap_off;
   int fast_ready_word = 0, fast_ready_shift = 0, fast_share_on = 0, heap_total = 0, heap_in_smem = 0;
   bool fast = false;
-  uint4 *ring = nullptr;
-  uint4 *d_score_log = nullptr;   // [T] tagged chosen-node score per placement attempt of the run-length batches
-  uint8_t *vt_cat = nullptr;      // per-group verdict table of k_commit_fast (FastParams::vt_*), sized for vt_entries
-  double *vt_score = nullptr;
-  int32_t *vt_gstamp = nullptr;   // sized for vt_stamps
-  size_t vt_entries = 0, vt_stamps = 0;
+  Buf<uint4> ring;
+  Buf<uint4> d_score_log;         // [T] tagged chosen-node score per placement attempt of the run-length batches
+  Buf<uint8_t> vt_cat;            // per-group verdict table of k_commit_fast (FastParams::vt_*)
+  Buf<double> vt_score;
+  Buf<int32_t> vt_gstamp;
   int last_full = 0, last_incr = 0;
   // ---- HyperNode tree (vc_snapshot_set_topology) ----
   bool has_topo = false;
@@ -194,34 +242,31 @@ struct vc_snapshot {
   std::vector<uint8_t> h_job_soft;
   bool topo_any = false;  // the plugin scores pods of soft-mode topology jobs in this session
   Slot<int32_t> hn_up, hn_tier_s, hn_parent_s, job_soft_s, job_alloc0_s, placed_off_s, placed0_s, placed_n0_s;
-  int32_t *rep_placed = nullptr, *d_job_alloc = nullptr;
-  size_t rep_placed_count = 0, placed_total = 0;
+  Buf<int32_t> rep_placed, d_job_alloc;
+  size_t placed_total = 0;
   int topo_nval = 0;
   double topo_val[VC_MAX_TIERS + 2]{};
   Slot<int32_t> hn_member, hn_slot, cta_hn_off, cta_hn, node_chain, cta_chain_off, cta_chain;
   int chain_cap = 1, hn_smem = 0;
   Slot<double> hn_alloc, hn_used0;
-  double *rep_hn_used = nullptr;
-  size_t rep_hn_used_count = 0;
-  double *hn_score = nullptr;  // dense pass [G][H]
+  Buf<double> rep_hn_used;
+  Buf<double> hn_score;  // dense pass [G][H]
   // ---- device-only buffers ----
-  uint32_t *cstat = nullptr;
-  double *w_idle = nullptr, *w_used = nullptr, *w_pip = nullptr, *w_kreq = nullptr, *w_knz = nullptr;  // working copies
-  int32_t *w_pod_count = nullptr;
-  int32_t *rep_i32 = nullptr;
-  double *rep_f64 = nullptr;
-  HeapEnt *rep_heap = nullptr;
-  size_t rep_i32_stride = 0, rep_f64_stride = 0, rep_heap_stride = 0;
-  int rep_ctas = 0;  // CTA count the replica buffers were sized for
-  uint4 *mbox = nullptr;
-  long long *d_prof = nullptr, *d_wait = nullptr;
+  Buf<uint32_t> cstat;
+  Buf<double> w_idle, w_used, w_pip, w_kreq, w_knz;  // working copies
+  Buf<int32_t> w_pod_count;
+  Buf<int32_t> rep_i32;
+  Buf<double> rep_f64;
+  Buf<HeapEnt> rep_heap;
+  Buf<uint4> mbox;
+  Buf<long long> d_prof, d_wait;
   long long h_prof[16] = {0};
-  vc_decision *d_decisions = nullptr;
-  vc_visit *d_visits = nullptr;
-  int32_t *d_fit = nullptr, *d_counters = nullptr;
-  vc_decision *h_decisions = nullptr;  // pinned
-  vc_visit *h_visits = nullptr;
-  int32_t *h_fit = nullptr, *h_counters = nullptr;
+  Buf<vc_decision> d_decisions;
+  Buf<vc_visit> d_visits;
+  Buf<int32_t> d_fit, d_counters;
+  Buf<vc_decision, Mem::Pinned> h_decisions;
+  Buf<vc_visit, Mem::Pinned> h_visits;
+  Buf<int32_t, Mem::Pinned> h_fit, h_counters;
   int max_job_tasks = 1;
   int n_cta = 0, block = 0, npc = 0;
   size_t smem_bytes = 0;
@@ -233,23 +278,22 @@ struct vc_snapshot {
   // ---- dense pass (K1) ----
   bool dense_ready = false;
   int n_groups = 0, n_work = 0;
-  double *g_req = nullptr, *g_kreq = nullptr, *g_knz = nullptr, *g_order = nullptr, *g_best_score = nullptr;
-  uint32_t *g_has = nullptr;
-  int32_t *g_class = nullptr, *g_stats = nullptr, *g_best_node = nullptr;
-  uint8_t *g_cat = nullptr;
-  int32_t *work_group = nullptr, *work_begin = nullptr, *work_end = nullptr, *group_tasks = nullptr, *task_group = nullptr;
-  double *part_score = nullptr;
-  int32_t *part_node = nullptr;
-  uint32_t *mask_out = nullptr;
-  double *score_out = nullptr, *best_score = nullptr;
-  int32_t *best_node = nullptr;
+  Buf<double> g_order, g_best_score;
+  Buf<int32_t> g_stats, g_best_node;
+  Buf<uint8_t> g_cat;
+  Buf<int32_t> work_group, work_begin, work_end, group_tasks, task_group;
+  Buf<double> part_score;
+  Buf<int32_t> part_node;
+  Buf<uint32_t> mask_out;
+  Buf<double> score_out, best_score;
+  Buf<int32_t> best_node;
   int rows_per_item = 16;
   int mw32 = 0;        // 32-bit words per mask row on the device (16-byte pitch)
   int mw32_logical = 0;  // ... of the uint64 row the ABI hands out
-  double *g_final = nullptr;   // [G][Nloc] final score of every (group, node)
-  uint32_t *g_maskw = nullptr; // [G][mwg] feasibility words
+  Buf<double> g_final;    // [G][Nloc] final score of every (group, node)
+  Buf<uint32_t> g_maskw;  // [G][mwg] feasibility words
   int mwg = 0;
-  bool matrix_allocated = false;
+  bool matrix_allocated = false;  // score_out / mask_out are sized and zeroed for the tables of the last dense_prepare
   double last_expand_ms = 0, last_dense_ms = 0;
   // (the host copies of the task arrays the dense-pass grouping and the later actions read live in `ek`)
   // ---- backfill action (vc_snapshot_set_backfill / vc_backfill_run) ----
@@ -263,11 +307,10 @@ struct vc_snapshot {
   int evict_idx = 0;
   std::vector<int32_t> last_fit;  // allocate's fit-error list of the last vc_allocate_run
   std::vector<uint8_t> t_filtered;  // [T] 1: allocate left the task a NodesFitErrors entry with node errors
-  int *d_dbg = nullptr;
+  Buf<int> d_dbg;
   std::vector<int32_t> h_nominated;  // [T] node index per task or -1 (vc_snapshot_set_nominated); empty: none
   bool any_nominated = false;
-  int32_t *d_nominated = nullptr;
-  size_t d_nominated_cap = 0;
+  Buf<int32_t> d_nominated;
   bool fut_rows = false;  // Releasing / Pipelined resources present at open
   // ---- hierarchical drf (vc_snapshot_set_hdrf) ----
   bool hd_set = false;
@@ -275,14 +318,12 @@ struct vc_snapshot {
   std::vector<double> hd_weight, hd_jreq;
   vch::HdrfTree hd_tree;
   HdrfDev hdp{};            // device view of the tree, filled at upload (hdp.on: queue order by hdrf)
-  void *d_hd = nullptr;     // device copy of the tree tables
-  HdrfDev *d_hdp = nullptr; // device copy of hdp (with the replica slab of the last run)
-  unsigned char *rep_hd = nullptr;  // per-CTA tree replicas + queue heaps
-  size_t rep_hd_bytes = 0;
+  Buf<unsigned char> d_hd;  // device copy of the tree tables
+  Buf<HdrfDev> d_hdp;       // device copy of hdp (with the replica slab of the last run)
+  Buf<unsigned char> rep_hd;  // per-CTA tree replicas + queue heaps
   bool all_pure = true;  // every job's named roles map to one (class, request) group each: the role-keyed error cache is a no-op
   bool rows_integral = false;  // every quantity a placement adds to / subtracts from a node row is integer-valued
-  void *d_bf = nullptr;   // device slab of the backfill inputs / outputs
-  size_t d_bf_bytes = 0;
+  Buf<unsigned char> d_bf;  // device slab of the backfill inputs / outputs
   // ---- preempt / reclaim actions (vc_snapshot_set_running / vc_preempt_run / vc_reclaim_run) ----
   vch::RunningTasks rt;            // host copy of node.Tasks
   std::vector<uint32_t> t_flags;   // VC_TASK_* per pending task
@@ -290,32 +331,45 @@ struct vc_snapshot {
   vch::EvictSession es;            // session state as the actions so far left it
   bool es_built = false;
   std::vector<vc_visit> last_vis;  // visits of the last vc_allocate_run
-  double *w_rel = nullptr;         // working copy of Releasing (Statement.Evict adds to it)
-  void *d_ev = nullptr;            // device slab: running-task table + per-preemptor scratch
-  size_t d_ev_bytes = 0;
-  int32_t *h_ev = nullptr;         // mapped pinned: [0..EV_PICK_K) picked nodes, [EV_CMD_OFF..] apply command
+  Buf<double> w_rel;               // working copy of Releasing (Statement.Evict adds to it)
+  Buf<unsigned char> d_ev;         // device slab of the session, laid out once by ensure_evict_session:
+  struct {
+    int32_t *rt_off, *rt_idx;      // the running-task table
+    double *rt_req, *rt_kreq, *rt_knz;
+    uint32_t *rt_flags;
+    int32_t *rt_job;
+    uint8_t *rt_evicted;
+    int32_t *rt_prio, *j_ready;    // ReadyTaskNum per job, proportion's "queue above deserved"
+    uint8_t *q_over;
+    unsigned long long *key[2];    // two ranking scratch sets: the preemptor under trial and the one ranked ahead
+    uint8_t *cand[2];
+    int32_t *list[2], *samp;       // k_evict_samp: lists, counts, indexes
+    unsigned long long *soft;      // soft-taint maximum per ranking set (EvictParams::soft_word)
+    double *hn_used;               // network-topology-aware binpacking: hyperNodeResourceCache.used, the running tasks'
+    uint32_t *rt_has;              // presence bits, the plugin's node score per ranking set (no room without it)
+    double *nta[2];
+  } ev{};
+  Buf<int32_t, Mem::Mapped> h_ev;  // [0..EV_PICK_K) picked nodes, [EV_CMD_OFF..] apply command
   // preempt's arguments (vc_snapshot_set_preempt_options) and the topology-aware reading's device state
   vc_preempt_options popt{0, 10, 1, 100, 0, 0, 0, nullptr, nullptr};
   std::vector<int32_t> popt_prio;
   std::vector<int64_t> popt_start;
-  void *d_topo = nullptr;          // device slab: running-task keys, drf job state, per-node dry-run results and scratch
-  size_t d_topo_bytes = 0;
-  int32_t *h_topo = nullptr;       // mapped pinned: k_evict_select's hand-out, EV_TOPO_SEQ = its sequence word
+  Buf<unsigned char> d_topo;       // device slab: running-task keys, drf job state, per-node dry-run results and scratch
+  Buf<int32_t, Mem::Mapped> h_topo;  // k_evict_select's hand-out, EV_TOPO_SEQ = its sequence word
   // the pdb and cdp votes' table (vc_snapshot_set_victim_guards) and its device copy
   bool guards_set = false;
   vch::VictimGuards guards;
-  void *d_guard = nullptr;
-  size_t d_guard_bytes = 0;
+  Buf<unsigned char> d_guard;
   // ---- one session across the GPUs of a node (vc_comm_create / vc_comm_attach) ----
   int world = 1, rank = 0;
   int n_cta_total = 0;             // CTAs of all ranks (the exchange); n_cta stays this rank's grid
-  unsigned char *comm = nullptr;   // this rank's slab: mailbox | ring | score log (cudaMalloc, exported over CUDA IPC)
-  size_t comm_bytes = 0, comm_mbox_bytes = 0, comm_ring_off = 0, comm_log_off = 0, comm_bytes_all = 0;
+  Buf<unsigned char> comm;         // this rank's slab: mailbox | ring | score log (exported over CUDA IPC)
+  size_t comm_ring_off = 0, comm_log_off = 0, comm_bytes_all = 0;
   unsigned char *peer_comm[8] = {nullptr};  // every rank's slab as mapped into this process (own one included)
   bool comm_attached = false;
   // ---- incremental upload (vc_snapshot_update_nodes) ----
-  unsigned char *delta_pin = nullptr, *delta_dev = nullptr;
-  size_t delta_cap = 0;
+  Buf<unsigned char, Mem::Pinned> delta_pin;
+  Buf<unsigned char> delta_dev;
 };
 
 namespace {
@@ -324,7 +378,7 @@ template <class T>
 void put(vc_snapshot *s, Slot<T> &slot, const T *src, size_t count, bool plan) {
   if (plan) {
     slot.count = count;
-    slot.off = s->in.reserve(count * sizeof(T));
+    slot.off = s->in.take(count * sizeof(T));
   } else if (count) {
     if (src) std::memcpy(slot.h(s->in), src, count * sizeof(T));
     else std::memset(slot.h(s->in), 0, count * sizeof(T));
@@ -455,22 +509,16 @@ void choose_geometry(vc_snapshot *s) {
   }
 }
 
-int free_dense(vc_snapshot *s) {
-  if (s->g_final) cudaFree(s->g_final);
-  if (s->g_maskw) cudaFree(s->g_maskw);
-  s->g_final = nullptr; s->g_maskw = nullptr;
-  void *ptrs[] = {s->g_req, s->g_kreq, s->g_knz, s->g_order, s->g_best_score, s->g_has, s->g_class, s->g_stats,
-                  s->g_best_node, s->g_cat, s->work_group, s->work_begin, s->work_end, s->group_tasks, s->task_group,
-                  s->part_score, s->part_node, s->mask_out, s->score_out, s->best_score, s->best_node};
-  for (void *p : ptrs)
-    if (p) cudaFree(p);
-  s->g_req = s->g_kreq = s->g_knz = s->g_order = s->g_best_score = nullptr;
-  s->g_has = nullptr; s->g_class = s->g_stats = s->g_best_node = nullptr; s->g_cat = nullptr;
-  s->work_group = s->work_begin = s->work_end = s->group_tasks = s->task_group = nullptr;
-  s->part_score = nullptr; s->part_node = nullptr;
-  s->mask_out = nullptr; s->score_out = s->best_score = nullptr; s->best_node = nullptr;
-  s->dense_ready = false;
-  s->matrix_allocated = false;
+// the working node rows (w_*) back at the uploaded ones: an action's kernels move the working copies, the upload stays
+// intact for re-runs and the dense pass
+int reset_work_rows(vc_snapshot *s) {
+  const size_t N = s->dims.n_nodes, R = s->dims.n_dims, K = s->dims.n_kdims;
+  CUDA_TRY(cudaMemcpyAsync(s->w_idle, s->n_idle.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(s->w_used, s->n_used.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(s->w_pip, s->n_pip.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(s->w_kreq, s->n_kreq.d(s->in), K * N * 8, cudaMemcpyDeviceToDevice, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(s->w_knz, s->n_knz.d(s->in), 2 * N * 8, cudaMemcpyDeviceToDevice, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(s->w_pod_count, s->n_pod_count.d(s->in), N * 4, cudaMemcpyDeviceToDevice, s->stream));
   return VC_OK;
 }
 
@@ -533,17 +581,8 @@ int vc_snapshot_create(const vc_dims *dims, vc_snapshot **out) {
 
 void vc_snapshot_destroy(vc_snapshot *s) {
   if (!s) return;
-  free_dense(s);
   for (int r = 0; r < s->world; ++r)
     if (r != s->rank && s->peer_comm[r]) cudaIpcCloseMemHandle(s->peer_comm[r]);
-  if (s->comm) cudaFree(s->comm);
-  void *dptrs[] = {s->in.dev, s->cstat, s->w_idle, s->w_used, s->w_pip, s->w_kreq, s->w_knz, s->w_pod_count,
-                   s->rep_i32, s->rep_f64, s->rep_heap, s->rep_hn_used, s->rep_placed, s->d_job_alloc, s->hn_score, s->mbox, s->ring, s->d_score_log, s->d_prof, s->d_wait, s->d_dbg, s->d_nominated, s->d_decisions, s->d_visits, s->d_fit, s->d_counters, s->d_bf, s->w_rel, s->d_ev, s->d_hd, s->rep_hd, s->d_hdp, s->d_topo, s->d_guard,
-                   s->vt_cat, s->vt_score, s->vt_gstamp};
-  for (void *p : dptrs) if (p) cudaFree(p);
-  void *hptrs[] = {s->in.pin, s->h_decisions, s->h_visits, s->h_fit, s->h_counters, s->h_ev, s->delta_pin, s->h_topo};
-  if (s->delta_dev) cudaFree(s->delta_dev);
-  for (void *p : hptrs) if (p) cudaFreeHost(p);
   if (s->ev0) cudaEventDestroy(s->ev0);
   if (s->ev1) cudaEventDestroy(s->ev1);
   if (s->ev2) cudaEventDestroy(s->ev2);
@@ -603,19 +642,14 @@ int vc_comm_create(vc_snapshot *s, int world, int rank, void *handle_out) {
   s->uploaded = false;  // the launch geometry depends on the number of ranks
   s->world = world; s->rank = rank; s->comm_attached = false;
   const size_t T = s->dims.n_tasks;
-  const size_t mbox = sizeof(uint4) * MBOX_STRIDE * 2 * 2048, ring = sizeof(uint4) * RING_STRIDE * RING_DEPTH;
-  s->comm_mbox_bytes = mbox;
-  s->comm_ring_off = (mbox + 255) & ~(size_t)255;
-  s->comm_log_off = (s->comm_ring_off + ring + 255) & ~(size_t)255;
-  const size_t bytes = s->comm_log_off + (T + 64) * sizeof(uint4);
-  s->comm_bytes_all = bytes;
-  if (!s->comm || s->comm_bytes < bytes) {
-    if (s->comm) cudaFree(s->comm);
-    s->comm = nullptr;
-    CUDA_TRY(cudaMalloc(&s->comm, bytes));
-    s->comm_bytes = bytes;
-  }
-  CUDA_TRY(cudaMemset(s->comm, 0, s->comm_bytes));
+  Layout lay;
+  lay.take(sizeof(uint4) * MBOX_STRIDE * 2 * 2048);
+  s->comm_ring_off = lay.take(sizeof(uint4) * RING_STRIDE * RING_DEPTH);
+  s->comm_log_off = lay.take((T + 64) * sizeof(uint4));
+  s->comm_bytes_all = lay.used;
+  int rc = s->comm.reserve(lay.used);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemset(s->comm, 0, s->comm.capacity()));
   cudaIpcMemHandle_t h;
   CUDA_TRY(cudaIpcGetMemHandle(&h, s->comm));
   static_assert(sizeof(cudaIpcMemHandle_t) == VC_COMM_HANDLE_BYTES, "IPC handle size");
@@ -1038,12 +1072,7 @@ int vc_snapshot_upload(vc_snapshot *s, const vc_nodes *nd, const vc_tasks *tk, c
       if (s->h_nominated[t] >= 0) s->any_nominated = true;
     }
     if (s->any_nominated) {
-      if (T > s->d_nominated_cap) {
-        if (s->d_nominated) cudaFree(s->d_nominated);
-        s->d_nominated = nullptr;
-        CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&s->d_nominated), T * 4));
-        s->d_nominated_cap = T;
-      }
+      if ((rc = s->d_nominated.reserve(T * 4))) return rc;
       CUDA_TRY(cudaMemcpyAsync(s->d_nominated, s->h_nominated.data(), T * 4, cudaMemcpyHostToDevice, s->stream));
     }
   }
@@ -1072,24 +1101,22 @@ int vc_snapshot_upload(vc_snapshot *s, const vc_nodes *nd, const vc_tasks *tk, c
     auto put_i = [&](const std::vector<int32_t> &v) { size_t o = iv.size(); iv.insert(iv.end(), v.begin(), v.end()); return o; };
     const size_t o_par = put_i(t.parent), o_coff = put_i(t.child_off), o_ch = put_i(t.child), o_jn = put_i(t.j_node),
                  o_qpo = put_i(t.q_path_off), o_qp = put_i(t.q_path), o_qi = put_i(q_init);
-    const size_t ibytes = (iv.size() * 4 + 15) & ~(size_t)15;
-    const size_t bytes = ibytes + (t.weight.size() + R * J) * 8;
-    if (s->d_hd) cudaFree(s->d_hd);
-    s->d_hd = nullptr;
-    CUDA_TRY(cudaMalloc(&s->d_hd, std::max<size_t>(bytes, 16)));
-    unsigned char *db = static_cast<unsigned char *>(s->d_hd);
-    CUDA_TRY(cudaMemcpy(db, iv.data(), iv.size() * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(db + ibytes, t.weight.data(), t.weight.size() * 8, cudaMemcpyHostToDevice));
-    if (R * J) CUDA_TRY(cudaMemcpy(db + ibytes + t.weight.size() * 8, s->hd_jreq.data(), R * J * 8, cudaMemcpyHostToDevice));
-    const int32_t *di = reinterpret_cast<const int32_t *>(db);
+    Layout lay;
+    const size_t o_int = lay.take(iv.size() * 4), o_weight = lay.take(t.weight.size() * 8), o_jreq = lay.take(R * J * 8);
+    if ((rc = s->d_hd.reserve(lay.used))) return rc;
+    unsigned char *db = s->d_hd;
+    CUDA_TRY(cudaMemcpy(db + o_int, iv.data(), iv.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(db + o_weight, t.weight.data(), t.weight.size() * 8, cudaMemcpyHostToDevice));
+    if (R * J) CUDA_TRY(cudaMemcpy(db + o_jreq, s->hd_jreq.data(), R * J * 8, cudaMemcpyHostToDevice));
+    const int32_t *di = at<const int32_t>(db, o_int);
     HdrfDev &h = s->hdp;
     h.ord = vch::hdrf_order(*conf);
     h.on = h.ord.hdrf_on;  // hdrf's queueOrderFn is dispatched only with drf's EnabledQueueOrder
     h.M = t.M; h.n_init = (int)q_init.size();
     h.parent = di + o_par; h.child_off = di + o_coff; h.child = di + o_ch; h.j_node = di + o_jn;
     h.q_path_off = di + o_qpo; h.q_path = di + o_qp; h.q_init = di + o_qi;
-    h.weight = reinterpret_cast<const double *>(db + ibytes);
-    h.j_req = h.weight + t.weight.size();
+    h.weight = at<const double>(db, o_weight);
+    h.j_req = at<const double>(db, o_jreq);
     for (size_t d = 0; d < VC_MAX_DIMS; ++d) {
       double acc = 0;
       if (d < R) for (size_t j = 0; j < J; ++j) acc += jb->allocated[d * J + j];
@@ -1265,17 +1292,7 @@ int vc_snapshot_upload(vc_snapshot *s, const vc_nodes *nd, const vc_tasks *tk, c
     put(s, s->job_alloc0_s, s->h_job_alloc.data(), s->topo_any ? s->h_job_alloc.size() : 0, plan);
     put(s, s->placed_off_s, placed_off.data(), placed_off.size(), plan); put(s, s->placed0_s, placed0.data(), placed0.size(), plan);
     put(s, s->placed_n0_s, placed_n0.data(), placed_n0.size(), plan);
-    if (plan) {
-      size_t need = (s->in.used + 255) & ~(size_t)255;
-      if (need > s->in.cap) {
-        if (s->in.dev) cudaFree(s->in.dev);
-        if (s->in.pin) cudaFreeHost(s->in.pin);
-        s->in.dev = s->in.pin = nullptr;
-        CUDA_TRY(cudaMalloc(&s->in.dev, need));
-        CUDA_TRY(cudaMallocHost(&s->in.pin, need));
-        s->in.cap = need;
-      }
-    }
+    if (plan && ((rc = s->in.dev.reserve(s->in.padded())) || (rc = s->in.pin.reserve(s->in.padded())))) return rc;
   }
   tick("staging memcpy");
   CUDA_TRY(cudaEventRecord(s->ev0, s->stream));
@@ -1283,16 +1300,9 @@ int vc_snapshot_upload(vc_snapshot *s, const vc_nodes *nd, const vc_tasks *tk, c
   s->h2d_bytes = (int64_t)s->in.used;
 
   // ---- device-only buffers --------------------------------------------------------------
-  auto ensure = [&](auto *&ptr, size_t bytes) -> int {
-    if (ptr) return VC_OK;
-    void *q = nullptr;
-    CUDA_TRY(cudaMalloc(&q, std::max<size_t>(bytes, 16)));
-    ptr = reinterpret_cast<std::remove_reference_t<decltype(ptr)>>(q);
-    return VC_OK;
-  };
-  if ((rc = ensure(s->cstat, C * N * 4))) return rc;
-  if ((rc = ensure(s->w_idle, R * N * 8)) || (rc = ensure(s->w_used, R * N * 8)) || (rc = ensure(s->w_pip, R * N * 8)) ||
-      (rc = ensure(s->w_kreq, K * N * 8)) || (rc = ensure(s->w_knz, 2 * N * 8)) || (rc = ensure(s->w_pod_count, N * 4)))
+  if ((rc = s->cstat.reserve(C * N * 4))) return rc;
+  if ((rc = s->w_idle.reserve(R * N * 8)) || (rc = s->w_used.reserve(R * N * 8)) || (rc = s->w_pip.reserve(R * N * 8)) ||
+      (rc = s->w_kreq.reserve(K * N * 8)) || (rc = s->w_knz.reserve(2 * N * 8)) || (rc = s->w_pod_count.reserve(N * 4)))
     return rc;
   // K0
   K0Params k0;
@@ -1419,30 +1429,26 @@ int vc_snapshot_update_nodes(vc_snapshot *s, int32_t n_dirty, const int32_t *nod
   }
   if (m > 0) {
     const size_t rows_n = 4 * R + 2 * K, bytes = rows_n * m * 8 + m * 4 + m * 4;
-    if (bytes > s->delta_cap) {
-      if (s->delta_pin) cudaFreeHost(s->delta_pin);
-      if (s->delta_dev) cudaFree(s->delta_dev);
-      s->delta_pin = s->delta_dev = nullptr;
+    if (bytes > s->delta_dev.capacity()) {  // grown with slack: a cluster's dirty sets are of similar sizes
       const size_t cap = std::max<size_t>(bytes * 2, 1 << 16);
-      CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&s->delta_pin), cap));
-      CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&s->delta_dev), cap));
-      s->delta_cap = cap;
+      int rc;
+      if ((rc = s->delta_pin.reserve(cap)) || (rc = s->delta_dev.reserve(cap))) return rc;
     }
-    double *v = reinterpret_cast<double *>(s->delta_pin);
+    double *v = at<double>(s->delta_pin, 0);
     auto put_rows = [&](size_t row0, const double *src, size_t nrows) {
       if (src) std::memcpy(v + row0 * m, src, nrows * m * 8);
       else std::memset(v + row0 * m, 0, nrows * m * 8);
     };
     put_rows(0, rows->idle, R); put_rows(R, rows->used, R); put_rows(2 * R, rows->releasing, R); put_rows(3 * R, rows->pipelined, R);
     put_rows(4 * R, rows->k8s_requested, K); put_rows(4 * R + K, rows->k8s_nonzero_requested, 2);
-    int32_t *pi = reinterpret_cast<int32_t *>(s->delta_pin + rows_n * m * 8);
+    int32_t *pi = at<int32_t>(s->delta_pin, rows_n * m * 8);
     std::memcpy(pi, rows->pod_count, m * 4);
     std::memcpy(pi + m, node_idx, m * 4);
     CUDA_TRY(cudaMemcpyAsync(s->delta_dev, s->delta_pin, bytes, cudaMemcpyHostToDevice, s->stream));
     NodeDeltaParams p;
     p.N = (int)N; p.R = (int)R; p.K = (int)K; p.n = (int)m;
-    p.vals = reinterpret_cast<const double *>(s->delta_dev);
-    p.pods = reinterpret_cast<const int32_t *>(s->delta_dev + rows_n * m * 8);
+    p.vals = at<const double>(s->delta_dev, 0);
+    p.pods = at<const int32_t>(s->delta_dev, rows_n * m * 8);
     p.idx = p.pods + m;
     p.idle = s->n_idle.d(s->in); p.used = s->n_used.d(s->in); p.rel = s->n_rel.d(s->in); p.pip = s->n_pip.d(s->in);
     p.kreq = s->n_kreq.d(s->in); p.knz = s->n_knz.d(s->in); p.pod_count = s->n_pod_count.d(s->in);
@@ -1497,7 +1503,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   if (!s->uploaded) return fail(VC_EINVAL, "vc_snapshot_upload must precede vc_allocate_run");
   const double t0 = now_ms();
   const vc_dims &D = s->dims;
-  const size_t N = D.n_nodes, T = D.n_tasks, J = D.n_jobs, Q = D.n_queues, R = D.n_dims, K = D.n_kdims, NR = D.n_roles;
+  const size_t N = D.n_nodes, T = D.n_tasks, J = D.n_jobs, Q = D.n_queues, R = D.n_dims, NR = D.n_roles;
   if (s->dd.node_begin != 0 || s->dd.node_end != (int)N)
     return fail(VC_EUNSUPPORTED, "the commit engine takes the full node axis (vc_comm_create cuts it over the ranks itself)");
   if (s->world > 1 && !s->comm_attached) return fail(VC_EINVAL, "vc_comm_attach must precede vc_allocate_run");
@@ -1511,70 +1517,32 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   // per-CTA heap replica: HeapEnt entries for k_commit, HeapKey (32 B) entries for k_commit_fast; stride in entries of
   // the kernel's own type, sized for the larger one
   const size_t heap_stride = (s->qjobs.count + 7) & ~(size_t)7;
-  if (!s->rep_i32 || s->rep_i32_stride != i32_stride || s->rep_f64_stride != f64_stride || s->rep_heap_stride != heap_stride ||
-      s->rep_ctas < G) {
-    if (s->rep_i32) cudaFree(s->rep_i32);
-    if (s->rep_f64) cudaFree(s->rep_f64);
-    if (s->rep_heap) cudaFree(s->rep_heap);
-    s->rep_i32 = nullptr; s->rep_f64 = nullptr; s->rep_heap = nullptr;
-    CUDA_TRY(cudaMalloc(&s->rep_i32, std::max<size_t>(16, i32_stride * G * 4)));
-    CUDA_TRY(cudaMalloc(&s->rep_f64, std::max<size_t>(16, f64_stride * G * 8)));
-    CUDA_TRY(cudaMalloc(&s->rep_heap, std::max<size_t>(16, std::max<size_t>(heap_stride, 1) * G * sizeof(HeapKey))));
-    s->rep_i32_stride = i32_stride; s->rep_f64_stride = f64_stride; s->rep_heap_stride = heap_stride;
-    s->rep_ctas = G;
-  }
-  if (s->topo_any && !s->d_job_alloc) CUDA_TRY(cudaMalloc(&s->d_job_alloc, std::max<size_t>(16, J * 4)));
-  if (s->topo_any) {
-    const size_t cnt = (size_t)G * std::max<size_t>(s->placed_total, 1);
-    if (!s->rep_placed || s->rep_placed_count < cnt) {
-      if (s->rep_placed) cudaFree(s->rep_placed);
-      s->rep_placed = nullptr;
-      CUDA_TRY(cudaMalloc(&s->rep_placed, cnt * 4));
-      s->rep_placed_count = cnt;
-    }
-  }
-  if (s->dc.nta_tables) {
-    const size_t cnt = (size_t)G * R * s->hn_cap;
-    if (!s->rep_hn_used || s->rep_hn_used_count < cnt) {
-      if (s->rep_hn_used) cudaFree(s->rep_hn_used);
-      s->rep_hn_used = nullptr;
-      CUDA_TRY(cudaMalloc(&s->rep_hn_used, std::max<size_t>(16, cnt * 8)));
-      s->rep_hn_used_count = cnt;
-    }
-  }
+  int rc;
+  if ((rc = s->rep_i32.reserve(i32_stride * G * 4)) || (rc = s->rep_f64.reserve(f64_stride * G * 8)) ||
+      (rc = s->rep_heap.reserve(std::max<size_t>(heap_stride, 1) * G * sizeof(HeapKey))))
+    return rc;
+  if (s->topo_any && ((rc = s->d_job_alloc.reserve(J * 4)) ||
+                      (rc = s->rep_placed.reserve((size_t)G * std::max<size_t>(s->placed_total, 1) * 4))))
+    return rc;
+  if (s->dc.nta_tables && (rc = s->rep_hn_used.reserve((size_t)G * R * s->hn_cap * 8))) return rc;
   const size_t mbox_bytes = kMboxBytes;
-  if (!s->mbox) CUDA_TRY(cudaMalloc(&s->mbox, mbox_bytes));
-  if (!s->d_prof) CUDA_TRY(cudaMalloc(&s->d_prof, 16 * sizeof(long long)));
   const size_t ring_bytes = sizeof(uint4) * RING_STRIDE * RING_DEPTH;
-  if (!s->ring) CUDA_TRY(cudaMalloc(&s->ring, ring_bytes));
-  if (!s->d_score_log) CUDA_TRY(cudaMalloc(&s->d_score_log, (T + 64) * sizeof(uint4)));
+  if ((rc = s->mbox.reserve(mbox_bytes)) || (rc = s->d_prof.reserve(16 * sizeof(long long))) ||
+      (rc = s->ring.reserve(ring_bytes)) || (rc = s->d_score_log.reserve((T + 64) * sizeof(uint4))))
+    return rc;
   // per-group verdict table: every (group, node slot of this rank) when the session fits the budget (not the SOFT instance)
   const size_t vt_entries = (size_t)s->n_groups * G * s->npc;
   const bool vt_on = s->fast && !s->dc.soft_active && vt_entries > 0 && vt_entries * 9 <= kVerdictTableBudget;
-  if (vt_on && s->vt_entries < vt_entries) {
-    if (s->vt_cat) cudaFree(s->vt_cat);
-    if (s->vt_score) cudaFree(s->vt_score);
-    s->vt_cat = nullptr; s->vt_score = nullptr; s->vt_entries = 0;
-    CUDA_TRY(cudaMalloc(&s->vt_cat, vt_entries));
-    CUDA_TRY(cudaMalloc(&s->vt_score, vt_entries * 8));
-    s->vt_entries = vt_entries;
-  }
-  if (vt_on && s->vt_stamps < (size_t)s->n_groups * G) {
-    if (s->vt_gstamp) cudaFree(s->vt_gstamp);
-    s->vt_gstamp = nullptr; s->vt_stamps = 0;
-    CUDA_TRY(cudaMalloc(&s->vt_gstamp, (size_t)s->n_groups * G * 4));
-    s->vt_stamps = (size_t)s->n_groups * G;
-  }
-  if (!s->d_decisions) {
-    CUDA_TRY(cudaMalloc(&s->d_decisions, std::max<size_t>(1, T) * sizeof(vc_decision)));
-    CUDA_TRY(cudaMalloc(&s->d_visits, (T + J + 1) * sizeof(vc_visit)));
-    CUDA_TRY(cudaMalloc(&s->d_fit, std::max<size_t>(1, T) * 4));
-    CUDA_TRY(cudaMalloc(&s->d_counters, kCounters * 4));
-    CUDA_TRY(cudaMallocHost(&s->h_decisions, std::max<size_t>(1, T) * sizeof(vc_decision)));
-    CUDA_TRY(cudaMallocHost(&s->h_visits, (T + J + 1) * sizeof(vc_visit)));
-    CUDA_TRY(cudaMallocHost(&s->h_fit, std::max<size_t>(1, T) * 4));
-    CUDA_TRY(cudaMallocHost(&s->h_counters, kCounters * 4));
-  }
+  if (vt_on && ((rc = s->vt_cat.reserve(vt_entries)) || (rc = s->vt_score.reserve(vt_entries * 8)) ||
+                (rc = s->vt_gstamp.reserve((size_t)s->n_groups * G * 4))))
+    return rc;
+  if ((rc = s->d_decisions.reserve(std::max<size_t>(1, T) * sizeof(vc_decision))) ||
+      (rc = s->d_visits.reserve((T + J + 1) * sizeof(vc_visit))) || (rc = s->d_fit.reserve(std::max<size_t>(1, T) * 4)) ||
+      (rc = s->d_counters.reserve(kCounters * 4)) ||
+      (rc = s->h_decisions.reserve(std::max<size_t>(1, T) * sizeof(vc_decision))) ||
+      (rc = s->h_visits.reserve((T + J + 1) * sizeof(vc_visit))) || (rc = s->h_fit.reserve(std::max<size_t>(1, T) * 4)) ||
+      (rc = s->h_counters.reserve(kCounters * 4)))
+    return rc;
   K2Params p;
   std::memset(&p, 0, sizeof p);
   p.d = s->dd; p.c = s->dc; p.npc = s->npc; p.n_cta = s->world > 1 ? s->n_cta_total : G; p.max_job_tasks = s->max_job_tasks;
@@ -1582,7 +1550,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   p.wd_cycles = (long long)(g_tun.watchdog_ms > 0 ? g_tun.watchdog_ms : 10000) * 2000000ll;  // ~2 GHz SM clock
   p.dbg = nullptr;
   if (g_tun.watchdog_ms > 0 && g_tun.prof) {  // diagnostics (VC_PROF=1 VC_WATCHDOG_MS=n): per-CTA progress words the watchdog prints
-    if (!s->d_dbg) CUDA_TRY(cudaMalloc(&s->d_dbg, 4096 * 32));
+    if ((rc = s->d_dbg.reserve(4096 * 32))) return rc;
     CUDA_TRY(cudaMemsetAsync(s->d_dbg, 0, 4096 * 32, s->stream));
     p.dbg = s->d_dbg;
   }
@@ -1592,7 +1560,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   p.req = s->t_req.d(s->in); p.tkreq = s->t_kreq.d(s->in); p.tknz = s->t_knz.d(s->in); p.req_has = s->t_has.d(s->in);
   p.t_class = s->t_class.d(s->in); p.t_role = s->t_role.d(s->in);
   p.task_order = s->task_order.d(s->in); p.job_task_off = s->job_task_off.d(s->in);
-  p.nominated = s->any_nominated ? s->d_nominated : nullptr;
+  p.nominated = s->any_nominated ? static_cast<int32_t *>(s->d_nominated) : nullptr;
   p.j_queue = s->j_queue.d(s->in); p.j_min = s->j_min.d(s->in); p.j_ntasks = s->j_ntasks.d(s->in);
   p.j_pbe = s->j_pbe.d(s->in); p.j_taskmintotal = s->j_taskmintotal.d(s->in); p.j_roleoff = s->j_roleoff.d(s->in);
   p.j_prio = s->j_prio.d(s->in); p.j_ready0 = s->j_ready0.d(s->in); p.j_waiting0 = s->j_waiting0.d(s->in);
@@ -1632,7 +1600,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
 
   long long *d_wait = nullptr;
   if (g_tun.prof_wait) {
-    if (!s->d_wait) CUDA_TRY(cudaMalloc(&s->d_wait, 1024 * 8));
+    if ((rc = s->d_wait.reserve(1024 * 8))) return rc;
     d_wait = s->d_wait;
     CUDA_TRY(cudaMemsetAsync(d_wait, 0, 1024 * 8, s->stream));
   }
@@ -1643,15 +1611,9 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
     HdrfDev hd = s->hdp;
     const size_t per = (((sizeof(HdrfAcc) + 15) & ~(size_t)15) + ((size_t)hd.M * R + hd.M + VC_MAX_DIMS) * 8 +
                         ((size_t)hd.M + J + Q + 1) * 4 + 15) & ~(size_t)15;
-    if (s->rep_hd_bytes < per * G) {
-      if (s->rep_hd) cudaFree(s->rep_hd);
-      s->rep_hd = nullptr;
-      CUDA_TRY(cudaMalloc(&s->rep_hd, per * G));
-      s->rep_hd_bytes = per * G;
-    }
+    if ((rc = s->rep_hd.reserve(per * G)) || (rc = s->d_hdp.reserve(sizeof(HdrfDev)))) return rc;
     hd.rep = s->rep_hd; hd.rep_stride = per;
     hd.q_prio = p.q_prio; hd.q_rank = p.q_rank;
-    if (!s->d_hdp) CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&s->d_hdp), sizeof(HdrfDev)));
     CUDA_TRY(cudaMemcpyAsync(s->d_hdp, &hd, sizeof hd, cudaMemcpyHostToDevice, s->stream));
     CUDA_TRY(cudaStreamSynchronize(s->stream));  // `hd` is a stack copy
     p.hd = s->d_hdp;
@@ -1678,12 +1640,12 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   fp.run_max = (s->rows_integral && !g_tun.commit_norun && s->dc.to_find == 0)
                    ? std::max(1, std::min(g_tun.run_max > 0 ? g_tun.run_max : RUN_MAX, std::min(RUN_MAX, 2 * (s->block / 32 - 1)))) : 1;
   fp.score_log = s->d_score_log;
-  fp.vt_cat = vt_on ? s->vt_cat : nullptr;
-  fp.vt_score = vt_on ? s->vt_score : nullptr;
-  fp.vt_gstamp = vt_on ? s->vt_gstamp : nullptr;
+  fp.vt_cat = vt_on ? static_cast<uint8_t *>(s->vt_cat) : nullptr;
+  fp.vt_score = vt_on ? static_cast<double *>(s->vt_score) : nullptr;
+  fp.vt_gstamp = vt_on ? static_cast<int32_t *>(s->vt_gstamp) : nullptr;
   if (s->world > 1) {  // mailbox, ring and score log live in the exported slabs; the score log is rank 0's (it writes the decisions)
-    p.mbox = reinterpret_cast<uint4 *>(s->comm);
-    p.ring = reinterpret_cast<uint4 *>(s->comm + s->comm_ring_off);
+    p.mbox = at<uint4>(s->comm, 0);
+    p.ring = at<uint4>(s->comm, s->comm_ring_off);
     for (int r = 0; r < s->world; ++r) {
       p.peer_mbox[r] = reinterpret_cast<uint4 *>(s->peer_comm[r]);
       p.peer_ring[r] = reinterpret_cast<uint4 *>(s->peer_comm[r] + s->comm_ring_off);
@@ -1700,13 +1662,7 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
     if (s->fast) CUDA_TRY(cudaMemsetAsync(s->d_score_log, 0, (T + 64) * sizeof(uint4), s->stream));
   }
   CUDA_TRY(cudaMemsetAsync(s->d_counters, 0, kCounters * 4, s->stream));
-  // working copies of the mutable node state (the uploaded snapshot stays intact for re-runs / K1)
-  CUDA_TRY(cudaMemcpyAsync(s->w_idle, s->n_idle.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(s->w_used, s->n_used.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(s->w_pip, s->n_pip.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(s->w_kreq, s->n_kreq.d(s->in), K * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(s->w_knz, s->n_knz.d(s->in), 2 * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(s->w_pod_count, s->n_pod_count.d(s->in), N * 4, cudaMemcpyDeviceToDevice, s->stream));
+  if ((rc = reset_work_rows(s))) return rc;
 
   void *args[] = {&p, &fp};
   CUDA_TRY(cudaLaunchCooperativeKernel(kfn, dim3(G), dim3(s->block), args, s->smem_bytes, s->stream));
@@ -1729,9 +1685,12 @@ int vc_allocate_run(vc_snapshot *s, vc_result **out) {
   if (n_fit) CUDA_TRY(cudaMemcpyAsync(s->h_fit, s->d_fit, (size_t)n_fit * 4, cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaStreamSynchronize(s->stream));
   vc_result *r = new vc_result();
-  r->decisions.assign(s->h_decisions, s->h_decisions + n_dec);
-  r->visits.assign(s->h_visits, s->h_visits + n_vis);
-  r->fit_errors.assign(s->h_fit, s->h_fit + n_fit);
+  const vc_decision *h_dec = s->h_decisions;
+  const vc_visit *h_vis = s->h_visits;
+  const int32_t *h_fit = s->h_fit;
+  r->decisions.assign(h_dec, h_dec + n_dec);
+  r->visits.assign(h_vis, h_vis + n_vis);
+  r->fit_errors.assign(h_fit, h_fit + n_fit);
   s->alloc_ran = true; s->bf_ran = false;
   s->last_dec = r->decisions;  // discarded visits carry no operations
   s->last_vis = r->visits;
@@ -1905,7 +1864,7 @@ namespace {
 // session state of the evicting actions: the opening session plus whatever vc_allocate_run did
 int ensure_evict_session(vc_snapshot *s) {
   const vc_dims &D = s->dims;
-  const size_t N = D.n_nodes, T = D.n_tasks, J = D.n_jobs, Q = D.n_queues, R = D.n_dims, K = D.n_kdims, NR = D.n_roles;
+  const size_t N = D.n_nodes, T = D.n_tasks, J = D.n_jobs, Q = D.n_queues, R = D.n_dims, K = D.n_kdims;
   if (s->bf.n > 0 || s->bf_ran) return fail(VC_EUNSUPPORTED, "preempt / reclaim: BestEffort pending tasks in the session");
   if (s->conf.min_nodes_to_find < 1 && N > 0 &&
       vch::num_feasible_nodes_to_find((int32_t)N, s->conf.percentage_nodes_to_find, s->conf.min_nodes_to_find,
@@ -1967,65 +1926,50 @@ int ensure_evict_session(vc_snapshot *s) {
   s->last_dec.clear();  // applied (a second evicting action continues from e)
   s->t_filtered = vch::fit_error_node_kinds(s->last_fit.data(), s->last_fit.size(), k.t_role.data(), k.r_flags.data(), T);
   // device: working rows (left by allocate, or the opening ones), Releasing, the running-task table, scratch
-  cudaError_t ce;
-  auto ensure = [&](auto *&ptr, size_t bytes) -> cudaError_t {
-    if (ptr) return cudaSuccess;
-    void *q = nullptr;
-    cudaError_t x = cudaMalloc(&q, std::max<size_t>(bytes, 16));
-    ptr = reinterpret_cast<std::remove_reference_t<decltype(ptr)>>(q);
-    return x;
-  };
-  if ((ce = ensure(s->w_rel, R * N * 8)) != cudaSuccess) return fail(VC_ECUDA, "cudaMalloc: %s", cudaGetErrorString(ce));
+  int rc;
+  if ((rc = s->w_rel.reserve(R * N * 8))) return rc;
   CUDA_TRY(cudaMemcpyAsync(s->w_rel, s->n_rel.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-  if (!s->alloc_ran) {
-    CUDA_TRY(cudaMemcpyAsync(s->w_idle, s->n_idle.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(s->w_used, s->n_used.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(s->w_pip, s->n_pip.d(s->in), R * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(s->w_kreq, s->n_kreq.d(s->in), K * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(s->w_knz, s->n_knz.d(s->in), 2 * N * 8, cudaMemcpyDeviceToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(s->w_pod_count, s->n_pod_count.d(s->in), N * 4, cudaMemcpyDeviceToDevice, s->stream));
-  }
+  if (!s->alloc_ran && (rc = reset_work_rows(s))) return rc;
   const size_t B = (size_t)std::max(s->rt.n, 1);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-  const size_t o_off = take((N + 1) * 4), o_idx = take(B * 4), o_req = take(R * B * 8), o_kreq = take(K * B * 8),
-               o_knz = take(K * B * 8), o_flags = take(B * 4), o_job = take(B * 4), o_ev = take(B), o_key = take(N * 8),
-               o_cand = take(N), o_prio = take(B * 4), o_jready = take(std::max<size_t>(J, 1) * 4), o_qover = take(std::max<size_t>(Q, 1)),
-               o_key2 = take(N * 8), o_cand2 = take(N),  // second ranking scratch: the preemptor ranked one ahead
-               o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4),  // k_evict_samp: lists, counts, indexes
-               o_soft = take(2 * 8),  // soft-taint maximum per ranking set (EvictParams::soft_word)
-               // network-topology-aware binpacking: hyperNodeResourceCache.used, the running tasks' presence bits, the
-               // plugin's node score per ranking set (sizes 0, so no room, without it)
-               o_hn = take(nta ? R * (size_t)s->hn_H * 8 : 0), o_has = take(nta ? B * 4 : 0), o_nta = take(nta ? N * 8 : 0),
-               o_nta2 = take(nta ? N * 8 : 0);
-  if (off > s->d_ev_bytes) {
-    if (s->d_ev) cudaFree(s->d_ev);
-    s->d_ev = nullptr;
-    CUDA_TRY(cudaMalloc(&s->d_ev, off));
-    s->d_ev_bytes = off;
-  }
-  if (!s->h_ev) CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&s->h_ev), (EV_CMD_OFF + 2 + EV_MAX_VICTIMS) * 4, cudaHostAllocMapped));
-  (void)o_key2; (void)o_cand2; (void)o_list; (void)o_list2; (void)o_samp; (void)o_soft; (void)o_nta; (void)o_nta2;
-  unsigned char *base = reinterpret_cast<unsigned char *>(s->d_ev);
-  CUDA_TRY(cudaMemsetAsync(base, 0, off, s->stream));
+  Layout lay;
+  const size_t o_off = lay.take((N + 1) * 4), o_idx = lay.take(B * 4), o_req = lay.take(R * B * 8), o_kreq = lay.take(K * B * 8),
+               o_knz = lay.take(K * B * 8), o_flags = lay.take(B * 4), o_job = lay.take(B * 4), o_ev = lay.take(B),
+               o_key = lay.take(N * 8), o_cand = lay.take(N), o_prio = lay.take(B * 4), o_jready = lay.take(std::max<size_t>(J, 1) * 4),
+               o_qover = lay.take(std::max<size_t>(Q, 1)), o_key2 = lay.take(N * 8), o_cand2 = lay.take(N),
+               o_list = lay.take(N * 4), o_list2 = lay.take(N * 4), o_samp = lay.take(8 * 4), o_soft = lay.take(2 * 8),
+               o_hn = lay.take(nta ? R * H * 8 : 0), o_has = lay.take(nta ? B * 4 : 0), o_nta = lay.take(nta ? N * 8 : 0),
+               o_nta2 = lay.take(nta ? N * 8 : 0);
+  if ((rc = s->d_ev.reserve(lay.padded())) || (rc = s->h_ev.reserve((EV_CMD_OFF + 2 + EV_MAX_VICTIMS) * 4))) return rc;
+  unsigned char *base = s->d_ev;
+  auto &v = s->ev;
+  v.rt_off = at<int32_t>(base, o_off); v.rt_idx = at<int32_t>(base, o_idx);
+  v.rt_req = at<double>(base, o_req); v.rt_kreq = at<double>(base, o_kreq); v.rt_knz = at<double>(base, o_knz);
+  v.rt_flags = at<uint32_t>(base, o_flags); v.rt_job = at<int32_t>(base, o_job); v.rt_evicted = base + o_ev;
+  v.key[0] = at<unsigned long long>(base, o_key); v.cand[0] = base + o_cand;
+  v.rt_prio = at<int32_t>(base, o_prio); v.j_ready = at<int32_t>(base, o_jready); v.q_over = base + o_qover;
+  v.key[1] = at<unsigned long long>(base, o_key2); v.cand[1] = base + o_cand2;
+  v.list[0] = at<int32_t>(base, o_list); v.list[1] = at<int32_t>(base, o_list2); v.samp = at<int32_t>(base, o_samp);
+  v.soft = at<unsigned long long>(base, o_soft);
+  v.hn_used = at<double>(base, o_hn); v.rt_has = at<uint32_t>(base, o_has);
+  v.nta[0] = at<double>(base, o_nta); v.nta[1] = at<double>(base, o_nta2);
+  CUDA_TRY(cudaMemsetAsync(base, 0, lay.padded(), s->stream));
   if (nta) {
-    CUDA_TRY(cudaMemcpyAsync(base + o_hn, hn_used.data(), R * H * 8, cudaMemcpyHostToDevice, s->stream));
-    if (s->rt.n > 0) CUDA_TRY(cudaMemcpyAsync(base + o_has, s->rt.has.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(v.hn_used, hn_used.data(), R * H * 8, cudaMemcpyHostToDevice, s->stream));
+    if (s->rt.n > 0) CUDA_TRY(cudaMemcpyAsync(v.rt_has, s->rt.has.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
   }
   if (s->rt.n > 0) {
     const vch::RunningTasks &b = s->rt;
-    CUDA_TRY(cudaMemcpyAsync(base + o_off, b.off.data(), (N + 1) * 4, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(base + o_idx, b.idx.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(base + o_req, b.req.data(), R * B * 8, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(base + o_kreq, b.kreq.data(), K * B * 8, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(base + o_knz, b.knz.data(), K * B * 8, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(base + o_flags, b.flags.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(base + o_job, b.job.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(base + o_prio, b.prio.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(v.rt_off, b.off.data(), (N + 1) * 4, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(v.rt_idx, b.idx.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(v.rt_req, b.req.data(), R * B * 8, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(v.rt_kreq, b.kreq.data(), K * B * 8, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(v.rt_knz, b.knz.data(), K * B * 8, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(v.rt_flags, b.flags.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(v.rt_job, b.job.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(v.rt_prio, b.prio.data(), B * 4, cudaMemcpyHostToDevice, s->stream));
   }
   CUDA_TRY(cudaStreamSynchronize(s->stream));
   s->es_built = true;
-  (void)NR; (void)o_ev; (void)o_key; (void)o_cand; (void)o_jready; (void)o_qover;
   return VC_OK;
 }
 
@@ -2058,33 +2002,18 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   // network-topology-aware with hypernode binpacking: every action books hyperNodeResourceCache.used (a reclaim can run
   // before a preempt on the same session); only preempt's normal reading ranks with the plugin's score
   const bool nta = s->dc.nta_on;
-  // device parameter block (same slab layout as ensure_evict_session)
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
-  const size_t o_off = take((N + 1) * 4), o_idx = take(B * 4), o_req = take(R * B * 8), o_kreq = take(K * B * 8),
-               o_knz = take(K * B * 8), o_flags = take(B * 4), o_job = take(B * 4), o_ev = take(B), o_key = take(N * 8),
-               o_cand = take(N), o_prio = take(B * 4), o_jready = take(std::max<size_t>(J, 1) * 4), o_qover = take(std::max<size_t>(Q, 1)),
-               o_key2 = take(N * 8), o_cand2 = take(N),  // second ranking scratch: the preemptor ranked one ahead
-               o_list = take(N * 4), o_list2 = take(N * 4), o_samp = take(8 * 4),  // k_evict_samp: lists, counts, indexes
-               o_soft = take(2 * 8),  // soft-taint maximum per ranking set (EvictParams::soft_word)
-               // network-topology-aware binpacking: hyperNodeResourceCache.used, the running tasks' presence bits, the
-               // plugin's node score per ranking set (sizes 0, so no room, without it)
-               o_hn = take(nta ? R * (size_t)s->hn_H * 8 : 0), o_has = take(nta ? B * 4 : 0), o_nta = take(nta ? N * 8 : 0),
-               o_nta2 = take(nta ? N * 8 : 0);
-  unsigned char *base = reinterpret_cast<unsigned char *>(s->d_ev);
+  const auto &v = s->ev;
   EvictParams p;
   std::memset(&p, 0, sizeof p);
   p.d = s->dd; p.c = s->dc;
   p.alloc = s->n_alloc.d(s->in); p.kalloc = s->n_kalloc.d(s->in);
   p.idle = s->w_idle; p.used = s->w_used; p.rel = s->w_rel; p.pip = s->w_pip; p.kreq = s->w_kreq; p.knz = s->w_knz;
   p.pod_count = s->w_pod_count; p.cstat = s->cstat;
-  p.rt_off = reinterpret_cast<const int32_t *>(base + o_off); p.rt_idx = reinterpret_cast<const int32_t *>(base + o_idx);
-  p.rt_req = reinterpret_cast<const double *>(base + o_req); p.rt_kreq = reinterpret_cast<const double *>(base + o_kreq);
-  p.rt_knz = reinterpret_cast<const double *>(base + o_knz); p.rt_flags = reinterpret_cast<const uint32_t *>(base + o_flags);
-  p.rt_job = reinterpret_cast<const int32_t *>(base + o_job); p.rt_evicted = base + o_ev;
+  p.rt_off = v.rt_off; p.rt_idx = v.rt_idx; p.rt_req = v.rt_req; p.rt_kreq = v.rt_kreq; p.rt_knz = v.rt_knz;
+  p.rt_flags = v.rt_flags; p.rt_job = v.rt_job; p.rt_evicted = v.rt_evicted;
   p.j_queue = s->j_queue.d(s->in); p.q_flags = s->q_flags.d(s->in); p.RT = (int)B;
-  p.rt_prio = reinterpret_cast<const int32_t *>(base + o_prio); p.j_prio = s->j_prio.d(s->in); p.j_min = s->j_min.d(s->in);
-  p.j_ready = reinterpret_cast<const int32_t *>(base + o_jready); p.q_over = base + o_qover;
+  p.rt_prio = v.rt_prio; p.j_prio = s->j_prio.d(s->in); p.j_min = s->j_min.d(s->in);
+  p.j_ready = v.j_ready; p.q_over = v.q_over;
   {
     double m1 = 0, m2 = 0;  // sums of requests are exact when every request is an integer well below 2^53 / RT
     p.exact_sums = (s->rows_integral && vch::max_abs_integral(s->rt.req.data(), s->rt.req.size(), m1) &&
@@ -2097,30 +2026,24 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     const vch::VictimGuards &g = s->guards;
     std::vector<uint8_t> bits(B, 0);
     for (int r = 0; r < g.n_running; ++r) bits[r] = g.device_bits(r);
-    size_t goff = 0;
-    auto gtake = [&](size_t bytes) { size_t o = goff; goff = (goff + bytes + 255) & ~(size_t)255; return o; };
-    const size_t g_bits = gtake(B), g_off = gtake((B + 1) * 4), g_pdb = gtake(std::max<size_t>(g.pdb.size(), 1) * 4),
-                 g_allowed = gtake(std::max<size_t>(g.allowed.size(), 1) * 4);
-    if (goff > s->d_guard_bytes) {
-      if (s->d_guard) cudaFree(s->d_guard);
-      s->d_guard = nullptr;
-      CUDA_TRY(cudaMalloc(&s->d_guard, goff));
-      s->d_guard_bytes = goff;
-    }
-    unsigned char *gb = reinterpret_cast<unsigned char *>(s->d_guard);
+    Layout lay;
+    const size_t g_bits = lay.take(B), g_off = lay.take((B + 1) * 4), g_pdb = lay.take(std::max<size_t>(g.pdb.size(), 1) * 4),
+                 g_allowed = lay.take(std::max<size_t>(g.allowed.size(), 1) * 4);
+    if ((rc = s->d_guard.reserve(lay.padded()))) return rc;
+    unsigned char *gb = s->d_guard;
     CUDA_TRY(cudaMemcpyAsync(gb + g_bits, bits.data(), B, cudaMemcpyHostToDevice, s->stream));
     CUDA_TRY(cudaMemcpyAsync(gb + g_off, g.off.data(), g.off.size() * 4, cudaMemcpyHostToDevice, s->stream));
     if (!g.pdb.empty()) CUDA_TRY(cudaMemcpyAsync(gb + g_pdb, g.pdb.data(), g.pdb.size() * 4, cudaMemcpyHostToDevice, s->stream));
     if (!g.allowed.empty())
       CUDA_TRY(cudaMemcpyAsync(gb + g_allowed, g.allowed.data(), g.allowed.size() * 4, cudaMemcpyHostToDevice, s->stream));
     d_rt_guard = gb + g_bits;
-    d_pdb_off = reinterpret_cast<const int32_t *>(gb + g_off); d_pdb = reinterpret_cast<const int32_t *>(gb + g_pdb);
-    d_pdb_allowed = reinterpret_cast<const int32_t *>(gb + g_allowed);
+    d_pdb_off = at<const int32_t>(gb, g_off); d_pdb = at<const int32_t>(gb, g_pdb);
+    d_pdb_allowed = at<const int32_t>(gb, g_allowed);
   }
   p.rt_guard = d_rt_guard;
   if (nta) {
     p.hn_H = s->hn_H; p.hn_member = s->hn_member.d(s->in); p.hn_alloc = s->hn_alloc.d(s->in);
-    p.hn_used = reinterpret_cast<double *>(base + o_hn); p.rt_has = reinterpret_cast<const uint32_t *>(base + o_has);
+    p.hn_used = v.hn_used; p.rt_has = v.rt_has;
   }
   // topology-aware preemption: the dry run's inputs beyond the ranking's, its per-node results and scratch
   const bool topo_on = !reclaim && s->popt.topology_aware;
@@ -2132,21 +2055,14 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   if (topo_on) {
     if (s->popt.n_running != s->rt.n)
       return fail(VC_EINVAL, "preempt options: %d pod priorities / start times for %d running tasks", s->popt.n_running, s->rt.n);
-    size_t toff = 0;
-    auto ttake = [&](size_t bytes) { size_t o = toff; toff = (toff + bytes + 255) & ~(size_t)255; return o; };
+    Layout lay;
     const size_t J1 = std::max<size_t>(J, 1);
-    const size_t t_rank = ttake(J1 * 4), t_pbe = ttake(J1 * 4), t_jalloc = ttake(R * J1 * 8), t_jshare = ttake(J1 * 8),
-                 t_podidx = ttake(B * 8), t_ts = ttake(B * 8), t_uid = ttake(B * 4), t_has = ttake(B * 4), t_pprio = ttake(B * 4),
-                 t_start = ttake(B * 8), t_a = ttake(B * 4), t_b = ttake(B * 4), t_f = ttake(B), t_g = ttake(B), t_ok = ttake(N),
-                 t_nv = ttake(N * 4), t_key = ttake(4 * N * 8);
-    if (toff > s->d_topo_bytes) {
-      if (s->d_topo) cudaFree(s->d_topo);
-      s->d_topo = nullptr;
-      CUDA_TRY(cudaMalloc(&s->d_topo, toff));
-      s->d_topo_bytes = toff;
-    }
-    if (!s->h_topo) CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&s->h_topo), (EV_TOPO_SEQ + 1) * 4, cudaHostAllocMapped));
-    unsigned char *tb = reinterpret_cast<unsigned char *>(s->d_topo);
+    const size_t t_rank = lay.take(J1 * 4), t_pbe = lay.take(J1 * 4), t_jalloc = lay.take(R * J1 * 8), t_jshare = lay.take(J1 * 8),
+                 t_podidx = lay.take(B * 8), t_ts = lay.take(B * 8), t_uid = lay.take(B * 4), t_has = lay.take(B * 4),
+                 t_pprio = lay.take(B * 4), t_start = lay.take(B * 8), t_a = lay.take(B * 4), t_b = lay.take(B * 4),
+                 t_f = lay.take(B), t_g = lay.take(B), t_ok = lay.take(N), t_nv = lay.take(N * 4), t_key = lay.take(4 * N * 8);
+    if ((rc = s->d_topo.reserve(lay.padded())) || (rc = s->h_topo.reserve((EV_TOPO_SEQ + 1) * 4))) return rc;
+    unsigned char *tb = s->d_topo;
     auto up = [&](size_t o, const void *src, size_t bytes) -> int {
       if (bytes) CUDA_TRY(cudaMemcpyAsync(tb + o, src, bytes, cudaMemcpyHostToDevice, s->stream));
       return VC_OK;
@@ -2168,28 +2084,28 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     tv.idle = s->w_idle; tv.rel = s->w_rel; tv.pip = s->w_pip;
     tv.rt_off = p.rt_off; tv.rt_idx = p.rt_idx; tv.rt_req = p.rt_req; tv.rt_flags = p.rt_flags; tv.rt_job = p.rt_job;
     tv.rt_prio = p.rt_prio; tv.rt_evicted = p.rt_evicted;
-    tv.rt_has = reinterpret_cast<const uint32_t *>(tb + t_has); tv.rt_uid = reinterpret_cast<const uint32_t *>(tb + t_uid);
-    tv.rt_podidx = reinterpret_cast<const int64_t *>(tb + t_podidx); tv.rt_ts = reinterpret_cast<const int64_t *>(tb + t_ts);
-    tv.rt_pod_prio = reinterpret_cast<const int32_t *>(tb + t_pprio); tv.rt_start = reinterpret_cast<const int64_t *>(tb + t_start);
+    tv.rt_has = at<const uint32_t>(tb, t_has); tv.rt_uid = at<const uint32_t>(tb, t_uid);
+    tv.rt_podidx = at<const int64_t>(tb, t_podidx); tv.rt_ts = at<const int64_t>(tb, t_ts);
+    tv.rt_pod_prio = at<const int32_t>(tb, t_pprio); tv.rt_start = at<const int64_t>(tb, t_start);
     tv.j_queue = p.j_queue; tv.j_prio = p.j_prio; tv.j_min = p.j_min; tv.j_ready = p.j_ready;
-    tv.j_pbe = reinterpret_cast<const int32_t *>(tb + t_pbe); tv.j_rank = reinterpret_cast<const uint32_t *>(tb + t_rank);
-    d_jalloc = reinterpret_cast<double *>(tb + t_jalloc); d_jshare = reinterpret_cast<double *>(tb + t_jshare);
+    tv.j_pbe = at<const int32_t>(tb, t_pbe); tv.j_rank = at<const uint32_t>(tb, t_rank);
+    d_jalloc = at<double>(tb, t_jalloc); d_jshare = at<double>(tb, t_jshare);
     tv.j_alloc = d_jalloc; tv.j_share = d_jshare;
     for (size_t d = 0; d < R; ++d) tv.total[d] = e.total[d];
     tv.total_has = e.total_has;
     tv.rt_guard = d_rt_guard; tv.pdb_off = d_pdb_off; tv.pdb = d_pdb; tv.pdb_allowed = d_pdb_allowed;
     tdry.cstat = s->cstat;
-    tdry.a = reinterpret_cast<int32_t *>(tb + t_a); tdry.b = reinterpret_cast<int32_t *>(tb + t_b);
+    tdry.a = at<int32_t>(tb, t_a); tdry.b = at<int32_t>(tb, t_b);
     tdry.f = tb + t_f; tdry.g = tb + t_g; tdry.ok = tb + t_ok;
-    tdry.nv = reinterpret_cast<int32_t *>(tb + t_nv); tdry.key = reinterpret_cast<long long *>(tb + t_key);
+    tdry.nv = at<int32_t>(tb, t_nv); tdry.key = at<long long>(tb, t_key);
   }
   // ReadyTaskNum per job and proportion's "queue above deserved" as the session stands; refreshed after every success
   std::vector<uint8_t> q_over(std::max<size_t>(Q, 1), 0);
   auto refresh_dynamic = [&]() -> int {
     for (size_t q = 0; q < Q; ++q)
       q_over[q] = (e.qattr[q].exists && !e.qattr[q].allocated.less_equal_zero(e.qattr[q].deserved, (int)R)) ? 1 : 0;
-    if (J) CUDA_TRY(cudaMemcpyAsync(base + o_jready, e.j_ready.data(), J * 4, cudaMemcpyHostToDevice, s->stream));
-    if (Q) CUDA_TRY(cudaMemcpyAsync(base + o_qover, q_over.data(), Q, cudaMemcpyHostToDevice, s->stream));
+    if (J) CUDA_TRY(cudaMemcpyAsync(v.j_ready, e.j_ready.data(), J * 4, cudaMemcpyHostToDevice, s->stream));
+    if (Q) CUDA_TRY(cudaMemcpyAsync(v.q_over, q_over.data(), Q, cudaMemcpyHostToDevice, s->stream));
     if (topo_on && J) {  // the dry run's drf votes and job order read the live allocations and shares
       CUDA_TRY(cudaMemcpyAsync(d_jalloc, e.j_alloc.data(), R * J * 8, cudaMemcpyHostToDevice, s->stream));
       CUDA_TRY(cudaMemcpyAsync(d_jshare, e.j_share.data(), J * 8, cudaMemcpyHostToDevice, s->stream));
@@ -2197,7 +2113,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     return VC_OK;
   };
   if ((rc = refresh_dynamic())) return rc;
-  p.key = reinterpret_cast<unsigned long long *>(base + o_key); p.cand = base + o_cand;
+  p.key = v.key[0]; p.cand = v.cand[0];
   int32_t *dev_h = nullptr;
   CUDA_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&dev_h), s->h_ev, 0));
   p.pick_node = dev_h; p.cmd = dev_h + EV_CMD_OFF;
@@ -2208,15 +2124,15 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   // its call left; d_samp[4] holds the index the action starts from. idx_live names the slot of the last call the action
   // consumed: a ranking made ahead scans from the preemptor under trial's slot and becomes live only when it is used.
   const bool samp = s->dc.to_find > 0;
-  int32_t *d_samp = reinterpret_cast<int32_t *>(base + o_samp);
-  int32_t *d_list[2] = {reinterpret_cast<int32_t *>(base + o_list), reinterpret_cast<int32_t *>(base + o_list2)};
+  int32_t *const d_samp = v.samp;
+  int32_t *const *d_list = v.list;
   int idx_live = 2;
   if (samp) CUDA_TRY(cudaMemcpyAsync(d_samp + 4, &s->evict_idx, 4, cudaMemcpyHostToDevice, s->stream));
   // PreferNoSchedule taints under TaintToleration's batch score change only the node order of preempt's normal reading
   // (reclaim and the topology-aware reading walk nodes without scores): those rankings take the SOFT instances, each
   // set's soft-taint maximum tagged with the sequence number of the ranking that wrote it (soft_seq[set])
   const bool soft = !reclaim && !topo_on && s->dc.soft_active;
-  unsigned long long *d_soft = reinterpret_cast<unsigned long long *>(base + o_soft);
+  unsigned long long *const d_soft = v.soft;
   unsigned long long soft_seq[2] = {0, 0}, soft_next = 0;
   int soft_klass[2] = {0, 0};
   if (soft) CUDA_TRY(cudaMemsetAsync(d_soft, 0, 2 * 8, s->stream));  // words left by an earlier action read as no maximum
@@ -2272,9 +2188,8 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   // discard in between (`epoch`) voids it. That includes network-topology-aware's hyperNodeResourceCache.used, which
   // only k_evict_apply moves: a ranking made ahead read the same hn_used as a ranking made now would.
   struct RankSet { unsigned long long *key; uint8_t *cand; int32_t *d_pick; volatile int32_t *h_pick; int seq; };
-  RankSet sets[2] = {{reinterpret_cast<unsigned long long *>(base + o_key), base + o_cand, dev_h, s->h_ev, 0},
-                     {reinterpret_cast<unsigned long long *>(base + o_key2), base + o_cand2, dev_h + (EV_PICK_K + 1),
-                      s->h_ev + (EV_PICK_K + 1), 0}};
+  RankSet sets[2] = {{v.key[0], v.cand[0], dev_h, s->h_ev, 0},
+                     {v.key[1], v.cand[1], dev_h + (EV_PICK_K + 1), s->h_ev + (EV_PICK_K + 1), 0}};
   s->h_ev[EV_PICK_K] = 0; s->h_ev[2 * EV_PICK_K + 1] = 0;
   int cur = 0, hint_t = -1, hint_mode = 0, pref_t = -1, pref_mode = 0, n_ahead = 0, n_ahead_used = 0;
   unsigned epoch = 0, pref_epoch = 0;
@@ -2283,7 +2198,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     EvictParams q = p;
     q.key = sets[k].key; q.cand = sets[k].cand; q.pick_node = sets[k].d_pick; q.samp_list = d_list[k]; q.samp_cnt = d_samp + k;
     q.soft_word = d_soft + k; q.soft_seq = soft_seq[k]; q.soft_klass = soft_klass[k]; q.soft_reduce = samp ? 0 : 1;
-    if (nta) q.nta_term = reinterpret_cast<double *>(base + (k ? o_nta2 : o_nta));
+    if (nta) q.nta_term = v.nta[k];
     return q;
   };
   auto launch_pick = [&](int k, int mode) -> int {
@@ -2465,7 +2380,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     };
   }
 
-  vc_result *r = new vc_result();
+  std::unique_ptr<vc_result> r(new vc_result());
   auto emit = [&](int job, const std::vector<vch::EvictOp> &ops, bool commit) {
     vc_visit v;
     v.job = job; v.first_op = (int32_t)r->decisions.size();
@@ -2479,7 +2394,6 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
       }
     r->visits.push_back(v);
   };
-  auto bail = [&](int code) { delete r; return code; };
   auto job_pending = [&](int j) { return (k.j_flags[j] & VC_JOB_PENDING_PHASE) && !e.phase_flipped; };
   auto pending_tasks = [&](int j, vch::GoPQ &pq) {
     pq.less = [&e](int l, int x) { return e.task_less(l, x); };
@@ -2515,12 +2429,12 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
           if (!e.job_starving(pj) || ptasks[pj].empty()) break;
           const int t = ptasks[pj].pop();
           if (!ptasks[pj].empty()) rk.hint(ptasks[pj].h[0], EV_MODE_PREEMPT_INTER);  // tried next unless this one succeeds
-          if ((rc = e.try_task(rk, stmt, t, EV_MODE_PREEMPT_INTER, &assigned))) return bail(rc);
+          if ((rc = e.try_task(rk, stmt, t, EV_MODE_PREEMPT_INTER, &assigned))) return rc;
         }
         if (e.job_pipelined(pj)) {
           emit(pj, stmt, true);
         } else {
-          if ((rc = e.discard_applied(rk, stmt))) return bail(rc);
+          if ((rc = e.discard_applied(rk, stmt))) return rc;
           emit(pj, stmt, false);
           continue;
         }
@@ -2533,9 +2447,9 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
           const int t = intra.pop();
           std::vector<vch::EvictOp> stmt;
           bool assigned = false;
-          if ((rc = e.try_task(rk, stmt, t, EV_MODE_PREEMPT_INTRA, &assigned))) return bail(rc);
+          if ((rc = e.try_task(rk, stmt, t, EV_MODE_PREEMPT_INTRA, &assigned))) return rc;
           if (!assigned) {
-            if ((rc = e.discard_applied(rk, stmt))) return bail(rc);
+            if ((rc = e.discard_applied(rk, stmt))) return rc;
             emit(j, stmt, false);
             break;
           }
@@ -2570,12 +2484,12 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
           if (!e.gate(VC_EN_PREEMPTIVE, q, t)) continue;           // ssn.Preemptive, reclaim.go:145-148
           if (!ptasks[job].empty()) rk.hint(ptasks[job].h[0], EV_MODE_RECLAIM);
           bool assigned = false;
-          if ((rc = e.try_task(rk, stmt, t, EV_MODE_RECLAIM, &assigned))) return bail(rc);
+          if ((rc = e.try_task(rk, stmt, t, EV_MODE_RECLAIM, &assigned))) return rc;
         }
         if (e.job_pipelined(job)) {
           emit(job, stmt, true);
         } else {
-          if ((rc = e.discard_applied(rk, stmt))) return bail(rc);
+          if ((rc = e.discard_applied(rk, stmt))) return rc;
           emit(job, stmt, false);
         }
         if (!preemptors[q].empty()) queues.push(q);
@@ -2583,9 +2497,8 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
     }
   }
   if (samp) {  // the index the last PredicateNodes call left, carried into the next action
-    cudaError_t ce = cudaMemcpyAsync(&s->evict_idx, d_samp + 2 + idx_live, 4, cudaMemcpyDeviceToHost, s->stream);
-    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s->stream);
-    if (ce != cudaSuccess) return bail(fail(VC_ECUDA, "evict index: %s", cudaGetErrorString(ce)));
+    CUDA_TRY(cudaMemcpyAsync(&s->evict_idx, d_samp + 2 + idx_live, 4, cudaMemcpyDeviceToHost, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));
     s->last_idx_cur = s->evict_idx;
   }
   r->stats.last_processed_node_index = samp ? s->evict_idx : s->last_idx_cur;
@@ -2597,7 +2510,7 @@ int run_evict_action(vc_snapshot *s, bool reclaim, vc_result **out) {
   r->stats.prof_cycles[1] = (int64_t)(t_sync * 1e3);
   r->stats.prof_cycles[2] = n_ahead;       // preemptors ranked one ahead / of those, how many rankings were used
   r->stats.prof_cycles[3] = n_ahead_used;
-  *out = r;
+  *out = r.release();
   return VC_OK;
 }
 
@@ -2665,27 +2578,23 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
   if (s->bf_ran) return fail(VC_EINVAL, "vc_backfill_run already ran on this session state (run vc_allocate_run or upload again)");
   const double t0 = now_ms();
   const vc_dims &D = s->dims;
-  const size_t N = D.n_nodes, T = D.n_tasks, J = D.n_jobs, Q = D.n_queues, R = D.n_dims, K = D.n_kdims, NR = D.n_roles;
+  const size_t N = D.n_nodes, T = D.n_tasks, J = D.n_jobs, Q = D.n_queues, R = D.n_dims, K = D.n_kdims;
   const size_t B = (size_t)s->bf.n;
-  vc_result *r = new vc_result();
+  std::unique_ptr<vc_result> r(new vc_result());
   r->stats.upload_ms = s->upload_ms;
-  if (B > 0 && s->dc.to_find > 0 && s->npc > 4 * s->block) { delete r; return fail(VC_EUNSUPPORTED, "feasible-node sampling: more than 4 x blockDim nodes per CTA"); }
-  if (B > 0 && samples_no_node(s)) {
-    delete r;
+  if (B > 0 && s->dc.to_find > 0 && s->npc > 4 * s->block) return fail(VC_EUNSUPPORTED, "feasible-node sampling: more than 4 x blockDim nodes per CTA");
+  if (B > 0 && samples_no_node(s))
     return fail(VC_EUNSUPPORTED, "backfill under feasible-node sampling: min-nodes-to-find below 1 and numNodesToFind 0");
-  }
   if (B > 0 && s->dc.nta_on) {
     // hypernode binpacking of a BestEffort pod: every term is skipped unless a weighted resource is requested
     // (network_topology_aware.go:507-520), i.e. unless "pods" is listed in hypernode.binpack.resources
     for (size_t t = 0; t < B; ++t)
       for (size_t d = 0; d < R; ++d)
-        if ((d < 2 || ((s->bf.has[t] >> d) & 1u)) && s->bf.req[d * B + t] >= vch::kMinRes && s->dc.nta_dim_weight[d] >= 0) {
-          delete r;
+        if ((d < 2 || ((s->bf.has[t] >> d) & 1u)) && s->bf.req[d * B + t] >= vch::kMinRes && s->dc.nta_dim_weight[d] >= 0)
           return fail(VC_EUNSUPPORTED, "backfill: network-topology-aware weighs a resource (dimension %zu) BestEffort pods request", d);
-        }
   }
-  if (s->dd.node_begin != 0 || s->dd.node_end != (int)N) { delete r; return fail(VC_EUNSUPPORTED, "the backfill engine runs on the full node axis"); }
-  if (B == 0) { *out = r; return VC_OK; }
+  if (s->dd.node_begin != 0 || s->dd.node_end != (int)N) return fail(VC_EUNSUPPORTED, "the backfill engine runs on the full node axis");
+  if (B == 0) { *out = r.release(); return VC_OK; }
   const vch::BackfillTasks &bf = s->bf;
   const vch::BackfillKeep &bk = s->bk;
   const vc_conf &conf = s->conf;
@@ -2736,27 +2645,14 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
   }
 
   // ---- 4. device buffers: one slab ----
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  size_t off = 0;
-  const size_t o_req = off; off += al(R * B * 8);
-  const size_t o_kreq = off; off += al(K * B * 8);
-  const size_t o_knz = off; off += al(2 * B * 8);
-  const size_t o_has = off; off += al(B * 4);
-  const size_t o_klass = off; off += al(B * 4);
-  const size_t o_group = off; off += al(B * 4);
-  const size_t o_order = off; off += al(std::max<size_t>(n, 1) * 4);
-  const size_t o_nta = off; off += al(nta_static.size() * 8);
-  const size_t in_bytes = off;
-  const size_t o_node = off; off += al(std::max<size_t>(n, 1) * 4);
-  const size_t o_score = off; off += al(std::max<size_t>(n, 1) * 8);
-  const size_t o_last = off; off += al(4);
-  const size_t o_prof = off; off += al(10 * 8);
-  if (s->d_bf_bytes < off) {
-    if (s->d_bf) cudaFree(s->d_bf);
-    s->d_bf = nullptr; s->d_bf_bytes = 0;
-    if (cudaMalloc(&s->d_bf, off) != cudaSuccess) { delete r; return fail(VC_ENOMEM, "backfill buffers (%zu bytes)", off); }
-    s->d_bf_bytes = off;
-  }
+  Layout lay;
+  const size_t o_req = lay.take(R * B * 8), o_kreq = lay.take(K * B * 8), o_knz = lay.take(2 * B * 8), o_has = lay.take(B * 4),
+               o_klass = lay.take(B * 4), o_group = lay.take(B * 4), o_order = lay.take(std::max<size_t>(n, 1) * 4),
+               o_nta = lay.take(nta_static.size() * 8);
+  const size_t in_bytes = lay.padded();
+  const size_t o_node = lay.take(std::max<size_t>(n, 1) * 4), o_score = lay.take(std::max<size_t>(n, 1) * 8),
+               o_last = lay.take(4), o_prof = lay.take(10 * 8);
+  if (s->d_bf.reserve(lay.padded())) return fail(VC_ENOMEM, "backfill buffers (%zu bytes)", lay.padded());
   std::vector<unsigned char> stage(in_bytes, 0);
   std::memcpy(stage.data() + o_req, bf.req.data(), R * B * 8);
   std::memcpy(stage.data() + o_kreq, bf.kreq.data(), K * B * 8);
@@ -2766,21 +2662,9 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
   std::memcpy(stage.data() + o_klass, bf.klass.data(), B * 4);
   std::memcpy(stage.data() + o_group, group.data(), B * 4);
   if (n) std::memcpy(stage.data() + o_order, order.data(), n * 4);
-  auto bail = [&](cudaError_t e, const char *what) {
-    delete r;
-    cudaGetLastError();  // a non-sticky error must not fail the next call's check
-    return fail(VC_ECUDA, "%s: %s", what, cudaGetErrorString(e));
-  };
-  cudaError_t e = cudaMemcpyAsync(s->d_bf, stage.data(), in_bytes, cudaMemcpyHostToDevice, s->stream);
-  if (e != cudaSuccess) return bail(e, "backfill H2D");
-  if (!s->alloc_ran) {  // no allocate action in this cycle: start from the opening node state
-    const struct { void *dst; const void *src; size_t bytes; } cp[] = {
-        {s->w_idle, s->n_idle.d(s->in), R * N * 8}, {s->w_used, s->n_used.d(s->in), R * N * 8},
-        {s->w_pip, s->n_pip.d(s->in), R * N * 8},   {s->w_kreq, s->n_kreq.d(s->in), K * N * 8},
-        {s->w_knz, s->n_knz.d(s->in), 2 * N * 8},   {s->w_pod_count, s->n_pod_count.d(s->in), N * 4}};
-    for (const auto &c : cp)
-      if ((e = cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToDevice, s->stream)) != cudaSuccess) return bail(e, "node state copy");
-  }
+  CUDA_TRY(cudaMemcpyAsync(s->d_bf, stage.data(), in_bytes, cudaMemcpyHostToDevice, s->stream));
+  int rc;
+  if (!s->alloc_ran && (rc = reset_work_rows(s))) return rc;  // no allocate action in this cycle: the opening node state
   float kms = 0;
   std::vector<int32_t> h_node(n, -1);
   std::vector<double> h_score(n, 0.0);
@@ -2789,8 +2673,8 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
   if (n > 0) {
     const int G = s->n_cta;
     const size_t mbox_bytes = kMboxBytes;
-    if (!s->mbox && (e = cudaMalloc(&s->mbox, mbox_bytes)) != cudaSuccess) return bail(e, "mailbox");
-    if ((e = cudaMemsetAsync(s->mbox, 0, mbox_bytes, s->stream)) != cudaSuccess) return bail(e, "mailbox reset");
+    if ((rc = s->mbox.reserve(mbox_bytes))) return rc;
+    CUDA_TRY(cudaMemsetAsync(s->mbox, 0, mbox_bytes, s->stream));
     K2Params p;
     std::memset(&p, 0, sizeof p);
     p.d = s->dd; p.c = s->dc; p.npc = s->npc; p.n_cta = G;
@@ -2800,7 +2684,7 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
     p.mbox = s->mbox;
     p.mbox2 = s->mbox + kMbox2Offset;
     BackfillParams bp;
-    unsigned char *base = static_cast<unsigned char *>(s->d_bf);
+    unsigned char *base = s->d_bf;
     bp.n = (int)n; bp.B = (int)B;
     bp.order = reinterpret_cast<const int32_t *>(base + o_order);
     bp.req = reinterpret_cast<const double *>(base + o_req); bp.kreq = reinterpret_cast<const double *>(base + o_kreq);
@@ -2815,21 +2699,21 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
                     : s->dc.soft_active ? (const void *)k_backfill<true> : (const void *)k_backfill<false>;
     const size_t smem = ((sizeof(BfCtl) + 15) & ~(size_t)15) + (3 * R + 2 * K + 2) * (size_t)s->npc * 8 +
                         (size_t)s->npc * (4 + 4) + 8 + (size_t)s->npc * (8 + 4 + 1 + 1) + 8 + (size_t)G * (8 + 4 + 4) + 64;
-    if ((e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return bail(e, "backfill smem");
+    CUDA_TRY(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int max_blocks = 0;
-    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_blocks, kfn, s->block, smem)) != cudaSuccess) return bail(e, "occupancy");
-    if (max_blocks * g_sm_count < G) { delete r; return fail(VC_EUNSUPPORTED, "backfill kernel cannot be co-resident: %d CTAs x %zu B smem", G, smem); }
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_blocks, kfn, s->block, smem));
+    if (max_blocks * g_sm_count < G) return fail(VC_EUNSUPPORTED, "backfill kernel cannot be co-resident: %d CTAs x %zu B smem", G, smem);
     void *args[] = {&p, &bp};
-    cudaEventRecord(s->ev0, s->stream);
-    if ((e = cudaLaunchCooperativeKernel(kfn, dim3(G), dim3(s->block), args, smem, s->stream)) != cudaSuccess) return bail(e, "backfill launch");
+    CUDA_TRY(cudaEventRecord(s->ev0, s->stream));
+    CUDA_TRY(cudaLaunchCooperativeKernel(kfn, dim3(G), dim3(s->block), args, smem, s->stream));
     g_launches++;
-    cudaEventRecord(s->ev1, s->stream);
-    if ((e = cudaMemcpyAsync(h_node.data(), base + o_node, n * 4, cudaMemcpyDeviceToHost, s->stream)) != cudaSuccess) return bail(e, "backfill D2H");
-    if ((e = cudaMemcpyAsync(h_score.data(), base + o_score, n * 8, cudaMemcpyDeviceToHost, s->stream)) != cudaSuccess) return bail(e, "backfill D2H");
-    if ((e = cudaMemcpyAsync(&h_last, base + o_last, 4, cudaMemcpyDeviceToHost, s->stream)) != cudaSuccess) return bail(e, "backfill D2H");
-    if (bp.prof && (e = cudaMemcpyAsync(h_prof, base + o_prof, 10 * 8, cudaMemcpyDeviceToHost, s->stream)) != cudaSuccess) return bail(e, "backfill D2H");
+    CUDA_TRY(cudaEventRecord(s->ev1, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(h_node.data(), base + o_node, n * 4, cudaMemcpyDeviceToHost, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(h_score.data(), base + o_score, n * 8, cudaMemcpyDeviceToHost, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(&h_last, base + o_last, 4, cudaMemcpyDeviceToHost, s->stream));
+    if (bp.prof) CUDA_TRY(cudaMemcpyAsync(h_prof, base + o_prof, 10 * 8, cudaMemcpyDeviceToHost, s->stream));
   }
-  if ((e = cudaStreamSynchronize(s->stream)) != cudaSuccess) return bail(e, "backfill kernel");
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
   if (n > 0) cudaEventElapsedTime(&kms, s->ev0, s->ev1);
   for (int k = 0; k < 8; ++k) r->stats.prof_cycles[k] = h_prof[k];
   if (g_tun.prof && n > 0)
@@ -2870,8 +2754,7 @@ int vc_backfill_run(vc_snapshot *s, vc_result **out) {
   r->stats.d2h_bytes = (int64_t)n * 12;
   r->stats.kernel_launches = n > 0 ? 1 : 0;
   r->stats.n_steps = (int32_t)n;
-  *out = r;
-  (void)NR;
+  *out = r.release();
   return VC_OK;
 }
 
@@ -2883,25 +2766,13 @@ __global__ void k_best_to_tasks(const int32_t *task_group, const double *g_best_
 
 static int dense_prepare(vc_snapshot *s) {
   if (s->dense_ready) return VC_OK;
-  free_dense(s);
+  s->matrix_allocated = false;
   const vc_dims &D = s->dims;
-  const size_t T = D.n_tasks, R = D.n_dims, K = D.n_kdims, N = D.n_nodes;
+  const size_t T = D.n_tasks, N = D.n_nodes;
   const int nloc = s->dd.node_end - s->dd.node_begin;
   const std::vector<int32_t> &group_of = s->h_group_of;
-  const std::vector<int32_t> &rep = s->group_rep;
-  const size_t G = rep.size();
-  s->n_groups = (int)G;
-  std::vector<double> g_req(R * G), g_kreq(K * G), g_knz(2 * G);
-  std::vector<uint32_t> g_has(G);
-  std::vector<int32_t> g_class(G), g_count(G + 1, 0);
-  for (size_t g = 0; g < G; ++g) {
-    int t = rep[g];
-    for (size_t d = 0; d < R; ++d) g_req[d * G + g] = s->ek.t_req[d * T + t];
-    for (size_t k = 0; k < K; ++k) g_kreq[k * G + g] = s->ek.t_kreq[k * T + t];
-    for (size_t k = 0; k < 2; ++k) g_knz[k * G + g] = s->ek.t_knz[k * T + t];
-    g_has[g] = s->ek.t_has[t] | ((s->topo_any && s->h_job_soft[s->ek.t_job[t]]) ? VC_HAS_TOPO_TASK : 0u);
-    g_class[g] = s->ek.t_class[t];
-  }
+  const size_t G = s->n_groups;  // the (class, request) groups of the upload, whose tables (sg_*) the pass reads
+  std::vector<int32_t> g_count(G + 1, 0);
   for (size_t t = 0; t < T; ++t) g_count[group_of[t] + 1]++;
   for (size_t g = 0; g < G; ++g) g_count[g + 1] += g_count[g];
   std::vector<int32_t> group_tasks(T), fill(g_count.begin(), g_count.end() - 1);
@@ -2926,35 +2797,24 @@ static int dense_prepare(vc_snapshot *s) {
   }
   s->n_work = (int)wg.size();
   s->rows_per_item = chunk;
-  auto up = [&](auto *&dptr, const auto &vec) -> int {
-    using E = typename std::remove_reference_t<decltype(vec)>::value_type;
-    void *q = nullptr;
-    CUDA_TRY(cudaMalloc(&q, std::max<size_t>(16, vec.size() * sizeof(E))));
-    if (!vec.empty()) CUDA_TRY(cudaMemcpyAsync(q, vec.data(), vec.size() * sizeof(E), cudaMemcpyHostToDevice, s->stream));
-    dptr = reinterpret_cast<std::remove_reference_t<decltype(dptr)>>(q);
+  auto up = [&](Buf<int32_t> &dst, const std::vector<int32_t> &vec) -> int {
+    const int rc = dst.reserve(vec.size() * 4);
+    if (rc) return rc;
+    if (!vec.empty()) CUDA_TRY(cudaMemcpyAsync(dst, vec.data(), vec.size() * 4, cudaMemcpyHostToDevice, s->stream));
     return VC_OK;
   };
   int rc;
-  if ((rc = up(s->g_req, g_req)) || (rc = up(s->g_kreq, g_kreq)) || (rc = up(s->g_knz, g_knz)) || (rc = up(s->g_has, g_has)) ||
-      (rc = up(s->g_class, g_class)) || (rc = up(s->work_group, wg)) || (rc = up(s->work_begin, wb)) ||
-      (rc = up(s->work_end, we)) || (rc = up(s->group_tasks, group_tasks)) || (rc = up(s->task_group, group_of)))
+  if ((rc = up(s->work_group, wg)) || (rc = up(s->work_begin, wb)) || (rc = up(s->work_end, we)) ||
+      (rc = up(s->group_tasks, group_tasks)) || (rc = up(s->task_group, group_of)))
     return rc;
   CUDA_TRY(cudaStreamSynchronize(s->stream));  // the staging vectors die with this scope
-  const int nparts = (nloc + 255) / 256;
-  CUDA_TRY(cudaMalloc(&s->g_order, std::max<size_t>(16, G * (size_t)nloc * 8)));
-  CUDA_TRY(cudaMalloc(&s->g_cat, std::max<size_t>(16, G * (size_t)nloc)));
-  CUDA_TRY(cudaMalloc(&s->g_stats, std::max<size_t>(16, G * 4 * 4)));
-  CUDA_TRY(cudaMalloc(&s->g_best_score, std::max<size_t>(16, G * 8)));
-  CUDA_TRY(cudaMalloc(&s->g_best_node, std::max<size_t>(16, G * 4)));
-  CUDA_TRY(cudaMalloc(&s->part_score, std::max<size_t>(16, G * (size_t)std::max(nparts, 1) * 8)));
-  CUDA_TRY(cudaMalloc(&s->part_node, std::max<size_t>(16, G * (size_t)std::max(nparts, 1) * 4)));
-  CUDA_TRY(cudaMalloc(&s->best_score, std::max<size_t>(16, T * 8)));
-  CUDA_TRY(cudaMalloc(&s->best_node, std::max<size_t>(16, T * 4)));
-  if (s->dc.nta_on) {
-    if (s->hn_score) cudaFree(s->hn_score);
-    s->hn_score = nullptr;
-    CUDA_TRY(cudaMalloc(&s->hn_score, std::max<size_t>(16, G * (size_t)s->hn_H * 8)));
-  }
+  const size_t nparts = std::max(1, (nloc + 255) / 256);
+  if ((rc = s->g_order.reserve(G * (size_t)nloc * 8)) || (rc = s->g_cat.reserve(G * (size_t)nloc)) ||
+      (rc = s->g_stats.reserve(G * 4 * 4)) || (rc = s->g_best_score.reserve(G * 8)) || (rc = s->g_best_node.reserve(G * 4)) ||
+      (rc = s->part_score.reserve(G * nparts * 8)) || (rc = s->part_node.reserve(G * nparts * 4)) ||
+      (rc = s->best_score.reserve(T * 8)) || (rc = s->best_node.reserve(T * 4)))
+    return rc;
+  if (s->dc.nta_on && (rc = s->hn_score.reserve(G * (size_t)s->hn_H * 8))) return rc;
   s->mw32_logical = (int)(2 * ((N + 63) / 64));
   s->mw32 = (s->mw32_logical + 3) & ~3;
   s->dense_ready = true;
@@ -2969,8 +2829,8 @@ static K1Params dense_params(vc_snapshot *s) {
   p.rel = s->n_rel.d(s->in); p.pip = s->n_pip.d(s->in); p.kalloc = s->n_kalloc.d(s->in);
   p.kreq = s->n_kreq.d(s->in); p.knz = s->n_knz.d(s->in);
   p.max_tasks = s->n_max_tasks.d(s->in); p.pod_count = s->n_pod_count.d(s->in); p.cstat = s->cstat;
-  p.n_groups = s->n_groups; p.g_req = s->g_req; p.g_kreq = s->g_kreq; p.g_knz = s->g_knz; p.g_has = s->g_has;
-  p.g_class = s->g_class; p.g_order = s->g_order; p.g_cat = s->g_cat; p.g_stats = s->g_stats;
+  p.n_groups = s->n_groups; p.g_req = s->sg_req.d(s->in); p.g_kreq = s->sg_kreq.d(s->in); p.g_knz = s->sg_knz.d(s->in);
+  p.g_has = s->sg_has.d(s->in); p.g_class = s->sg_class.d(s->in); p.g_order = s->g_order; p.g_cat = s->g_cat; p.g_stats = s->g_stats;
   p.g_best_score = s->g_best_score; p.g_best_node = s->g_best_node;
   p.n_work = s->n_work; p.work_group = s->work_group; p.work_begin = s->work_begin; p.work_end = s->work_end;
   p.group_tasks = s->group_tasks; p.mask_out = s->mask_out; p.score_out = s->score_out;
@@ -3018,8 +2878,8 @@ int vc_dense_finish(vc_snapshot *s, int materialize) {
   const size_t T = D.n_tasks, N = D.n_nodes;
   const int nloc = s->dd.node_end - s->dd.node_begin;
   if (materialize && !s->matrix_allocated) {
-    CUDA_TRY(cudaMalloc(&s->score_out, std::max<size_t>(16, T * N * 8)));
-    CUDA_TRY(cudaMalloc(&s->mask_out, std::max<size_t>(16, T * (size_t)s->mw32 * 4)));
+    int rc;
+    if ((rc = s->score_out.reserve(T * N * 8)) || (rc = s->mask_out.reserve(T * (size_t)s->mw32 * 4))) return rc;
     CUDA_TRY(cudaMemsetAsync(s->score_out, 0, std::max<size_t>(16, T * N * 8), s->stream));
     CUDA_TRY(cudaMemsetAsync(s->mask_out, 0, std::max<size_t>(16, T * (size_t)s->mw32 * 4), s->stream));
     s->matrix_allocated = true;
@@ -3041,10 +2901,9 @@ int vc_dense_finish(vc_snapshot *s, int materialize) {
     if ((N % 2) == 0 && (s->dd.node_begin % 128) == 0 && !g_tun.expand_plain) {
       // bulk-copy variant: final rows of the groups first (G x Nloc evaluations), then one streaming kernel
       s->mwg = ((nloc + 127) / 128) * 4;
-      if (!s->g_final) {
-        CUDA_TRY(cudaMalloc(&s->g_final, std::max<size_t>(16, (size_t)s->n_groups * nloc * 8)));
-        CUDA_TRY(cudaMalloc(&s->g_maskw, std::max<size_t>(16, (size_t)s->n_groups * s->mwg * 4)));
-      }
+      int rc;
+      if ((rc = s->g_final.reserve((size_t)s->n_groups * nloc * 8)) || (rc = s->g_maskw.reserve((size_t)s->n_groups * s->mwg * 4)))
+        return rc;
       CUDA_TRY(cudaMemsetAsync(s->g_maskw, 0, std::max<size_t>(16, (size_t)s->n_groups * s->mwg * 4), s->stream));
       LAUNCH_Y_SLICED(k_group_final, (nloc + 255) / 256, s->n_groups, 256, 0, s->stream, p, s->g_final, s->g_maskw, s->mwg);
       g_launches++;
