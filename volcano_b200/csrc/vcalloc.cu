@@ -493,7 +493,9 @@ void choose_geometry(vc_snapshot *s) {
   s->fast = fast0;
   if (s->fast) {
     if (g_tun.commit_threads <= 0) s->block = 256;  // 7 worker warps: a run's node states are evaluated two per warp
-    size_t rows = 3 * (size_t)R + (s->dc.has_future ? 2 * (size_t)R : 0) + 2 * (size_t)K + 2 + 1;
+    // the Releasing / Pipelined rows exist in the FUT instances only (dc.has_future is also set by sampling, whose
+    // incremental instance without them is <.., FUT = false, .., SAMP>)
+    size_t rows = 3 * (size_t)R + (s->fut_rows ? 2 * (size_t)R : 0) + 2 * (size_t)K + 2 + 1;
     s->smem_bytes = ((sizeof(Ctl) + 15) & ~(size_t)15) + ((sizeof(CtlFast) + 15) & ~(size_t)15) + rows * npc * 8 +
                     (size_t)npc * (8 + 4 * 7) + (size_t)s->n_cta_total * (8 + 4 + 4 + 4 + 4) + 64;
     const size_t heap_bytes = (size_t)s->heap_total * sizeof(HeapKey);
@@ -1417,7 +1419,7 @@ int vc_snapshot_update_nodes(vc_snapshot *s, int32_t n_dirty, const int32_t *nod
   bool fut = false;
   for (size_t i = 0; i < R * m && !fut; ++i)
     if ((rows->releasing && rows->releasing[i] != 0.0) || (rows->pipelined && rows->pipelined[i] != 0.0)) fut = true;
-  if (fut && !s->dc.has_future)
+  if (fut && (s->fast ? !s->fut_rows : !s->dc.has_future))
     return fail(VC_EUNSUPPORTED, "incremental upload: first Releasing / Pipelined resource of the session, upload it in full");
   // every value the run-length batches rely on stays an integer of safe magnitude
   if (s->rows_integral) {
